@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- pose hypotheses / second through render + coarse + 5x refine (BASELINE.json metric).
 
-    python bench.py --gpus 1 --steps 5 --warmup 3            # this framework (libmpx.so, sm_100a)
+    python bench.py --gpus 1 --steps 5 --warmup 3            # this framework (libmpx.so, sm_90a)
+    python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs DIR   # + the last timed step's outputs as DIR/*.npy
     python bench.py --impl reference --steps 2 --warmup 1    # the reference path on the host cores (CPU oracle port)
     python bench.py --impl torch-gpu                         # the same networks through stock torch / cuDNN on this GPU
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ... [--scaling strong]
@@ -40,8 +41,8 @@ N_REFINER_ITERS = 5
 # SURVEY.md 8(d), FLOP = 2*MAC, conv + linear: {render size: (coarse/scoring forward, RGB refiner forward)} GFLOP per sample
 GFLOP = {(240, 320): (12.068, 14.236), (224, 224): (7.799, 9.215)}
 # 16-bit bytes the 36 convolutions of one coarse forward move at least once per hypothesis at 240x320 (each conv: input
-# read + output write + residual read; weights excluded): stem 2.46 MB in + 0.61 MB pooled out (the max-pool runs in its
-# epilogue; 2 x 2.46 MB before), layer1 6 convs of 60x80x64, ... = 26.42 MB
+# read + output write + residual read; weights excluded): stem 2.46 MB in + 0.61 MB pooled out (counting the max-pool as
+# fused into the stem's epilogue), layer1 6 convs of 60x80x64, ... = 26.42 MB
 ALGO_CONV_BYTES_PER_HYP = 26.42e6
 
 
@@ -67,6 +68,8 @@ def parse_args():
     ap.add_argument("--no-full-unit", action="store_true", help="CPU arm: skip the one complete 576-hypothesis unit")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-torch-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what run_inference_pipeline returned for the last timed step as DIR/<name>.npy")
     a = ap.parse_args()
     a.render_size = tuple(int(v) for v in a.render_size.lower().split("x"))
     assert a.render_size in GFLOP, f"--render-size must be one of {sorted(GFLOP)}"
@@ -96,7 +99,7 @@ def workload_config(args, sc, n_gpus: int):
                                 "frame i overlap the coarse stage of frame i+1 on a second stream; every frame's result is "
                                 "produced and read; `single_frame` has the one-blocking-call-per-step numbers)",
             "l2": f"network input tensor ({2 * 64 * (h // 2) * (w // 2) * M_GRID * B / n_gpus / 1e9:.2f} GB per rank and "
-                  "step) >> 126 MB L2, no explicit flush"}
+                  "step) >> 50 MB L2, no explicit flush"}
 
 
 def bbox_pool(bboxes, n=4):
@@ -201,7 +204,7 @@ def cpu_baseline_subprocess(args):
 
 
 # ---------------------------------------------------------------------------------------------
-# torch / cuDNN arm: the same two networks through stock PyTorch on this GPU (the "existing Blackwell kernel" bar)
+# torch / cuDNN arm: the same two networks through stock PyTorch on this GPU (the vendor-library bar)
 # ---------------------------------------------------------------------------------------------
 def torch_gpu_baseline(sc, quick: bool = False):
     """Network-only time of one config-2 unit through torch / cuDNN: coarse forward over 576 hypotheses (one batch, and in
@@ -295,6 +298,34 @@ class ClockSampler:
 
 
 # ---------------------------------------------------------------------------------------------
+# --dump-outputs: what the timed path returned for its last step, for output-for-output comparison of two builds
+# ---------------------------------------------------------------------------------------------
+def output_arrays(result) -> dict:
+    """(final, extra_data) of run_inference_pipeline -> {name: float32 / float64 array}: the final estimates' tensors and
+    numeric columns, the coarse logits of all hypotheses and the refined poses of every iteration (a few hundred KB)."""
+    import pandas as pd
+
+    final, extra = result
+    out = {f"final_{k}": v.detach().float().cpu().numpy() for k, v in final.tensors.items()}
+    for col in final.infos.columns:
+        if pd.api.types.is_numeric_dtype(final.infos[col]):
+            out[f"final_{col}"] = final.infos[col].to_numpy(dtype=np.float64)
+    out["coarse_logits"] = extra["coarse"]["data"]["logits"].detach().float().cpu().numpy()
+    for name, pred in extra["refiner_all_hypotheses"]["preds"].items():
+        out[f"refiner_{name.replace('=', '')}_poses"] = pred.poses.detach().float().cpu().numpy()
+    return out
+
+
+def write_outputs(arrays: dict, out_dir: str) -> None:
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= 64 << 20, f"--dump-outputs: {total} bytes exceed 64 MB"
+    for name, a in arrays.items():
+        np.save(d / f"{name}.npy", a)
+
+
+# ---------------------------------------------------------------------------------------------
 # GPU arm
 # ---------------------------------------------------------------------------------------------
 def run_mpx_arm(args):
@@ -337,6 +368,7 @@ def run_mpx_arm(args):
     images_dev, K_dev, pool_dev = images.cuda(), K.cuda(), [b.cuda() for b in pool]
     images_pin, K_pin, pool_pin = images.pin_memory(), K.pin_memory(), [b.pin_memory() for b in pool]
     counter = [0]
+    last = [None]  # (final, extra_data) of the most recent step
 
     kw = dict(n_refiner_iterations=N_REFINER_ITERS, n_pose_hypotheses=1)
 
@@ -354,13 +386,15 @@ def run_mpx_arm(args):
 
     def step_device(e=None):
         obs, det = frame_device()
-        return (e or est).run_inference_pipeline(obs, detections=det, **kw)[0]
+        last[0] = (e or est).run_inference_pipeline(obs, detections=det, **kw)
+        return last[0][0]
 
     def run_single(steps, host: bool):  # one blocking call per step
         for _ in range(steps):
             if host:
                 obs, det = frame_host()
-                read_back(est.run_inference_pipeline(obs, detections=det, **kw)[0])
+                last[0] = est.run_inference_pipeline(obs, detections=det, **kw)
+                read_back(last[0][0])
             else:
                 step_device()
 
@@ -370,10 +404,12 @@ def run_mpx_arm(args):
             done = pipe.submit(*(frame_host() if host else frame_device()), **kw)
             if done is not None:
                 n_done += 1
+                last[0] = done
                 if host:
                     read_back(done[0])
         for done in pipe.drain():
             n_done += 1
+            last[0] = done
             if host:
                 read_back(done[0])
         pipe.join()
@@ -406,6 +442,8 @@ def run_mpx_arm(args):
     if rank == 0:
         sampler.start()
     total_ms = timed(run, args.steps, False)
+    # copied before the next step can reuse the estimators' buffers
+    dumped = output_arrays(last[0]) if args.dump_outputs and rank == 0 else None
     run(2 * n_fif, True)
     e2e_ms = timed(run, args.steps, True)
     single = None
@@ -457,8 +495,9 @@ def run_mpx_arm(args):
             burst, sustained = float(peaks.get("bf16_tflops", 1700.0)), float(peaks.get("bf16_tflops_sustained", 1400.0))
             peak_src = "MEASURED_PEAKS.json bf16_tflops (burst: the timed region is a sub-second burst at full clocks)"
         else:
-            burst, sustained = 1700.0, 1400.0
-            peak_src = "fallback figures of B200_PROFILING.md (MEASURED_PEAKS.json absent)"
+            # dense fp16 / bf16 of the H100 SXM data sheet (a card allowed 700 W; a lower power limit lowers the clocks)
+            burst = sustained = 989.0
+            peak_src = "NVIDIA H100 SXM data sheet, dense fp16/bf16 (MEASURED_PEAKS.json absent): not reached by any kernel"
         conv_ms_per_step = conv_ms.value / prof_steps
         # The event-timed launches are the convolutions of this rank's coarse forward(s) (the refiner iterations and the
         # final scoring replay CUDA graphs, whose kernels are not individually timed): algorithmic work of exactly those
@@ -466,13 +505,6 @@ def run_mpx_arm(args):
         rows_rank = M_GRID * n_det / n_gpus
         algo_tflop_per_step = GFLOP[(h, w)][0] * rows_rank / 1000.0
         achieved = algo_tflop_per_step / (conv_ms_per_step / 1000.0)
-        traffic = None
-        tpath = ROOT / "profiles" / "conv_traffic.json"
-        if tpath.exists() and (h, w) == (240, 320) and rows_rank == M_GRID:
-            # dram__bytes_read.sum + dram__bytes_write.sum of the same 36 launches from one ncu pass of this workload (a
-            # constant read from the file, not a measurement of this run)
-            tj = json.loads(tpath.read_text())
-            traffic = float(tj["dram_read_bytes"]) + float(tj["dram_write_bytes"])
         line = {
             "metric": "pose hypotheses/sec through render+coarse+5x refine", "value": value, "unit": "hypotheses/s",
             "impl": "mpx", "n_gpus": n_gpus, "steps": args.steps, "warmup": warmup, "ms_per_step": ms_per_step,
@@ -490,13 +522,10 @@ def run_mpx_arm(args):
                 "e2e_value": hyp_per_step / (single[1] / args.steps / 1000.0), "unit": "hypotheses/s"},
             "clocks": clocks,
             "roofline": {"bound": "tensor",
-                         "kernel": "tcgen05 implicit-GEMM convolutions (conv_window / conv_igemm / conv_igemm2): the "
-                                   "launches of this rank's coarse forward, summed",
+                         "kernel": "wgmma implicit-GEMM convolutions (conv_wgmma_kernel): the launches of this rank's "
+                                   "coarse forward, summed",
                          "achieved": achieved, "peak": burst, "unit": "TFLOP/s", "frac": achieved / burst,
                          "frac_of_sustained_peak": achieved / sustained, "peak_sustained": sustained,
-                         "traffic": traffic,
-                         "traffic_source": "profiles/conv_traffic.json (one ncu pass of this workload; a constant, not a "
-                                           "measurement of this run)" if traffic is not None else None,
                          "algorithmic_activation_bytes": ALGO_CONV_BYTES_PER_HYP * rows_rank if (h, w) == (240, 320) else None,
                          "peak_source": peak_src, "algorithmic_tflop_per_step": algo_tflop_per_step,
                          "executed_tflop_per_step": conv_fl.value / prof_steps / 1e12,
@@ -514,6 +543,9 @@ def run_mpx_arm(args):
                 line["gpu_torch_baseline"] = {"failed": repr(exc)[:300]}
         if n_gpus == 1 and not args.no_cpu_baseline and args.workload == "rgb576":
             line["cpu_baseline"] = cpu_baseline_subprocess(args)
+        if dumped is not None:
+            write_outputs(dumped, args.dump_outputs)
+            line["dumped_outputs"] = {"dir": str(args.dump_outputs), "arrays": sorted(dumped)}
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()

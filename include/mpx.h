@@ -1,5 +1,5 @@
 /*
- * mpx.h -- C ABI of libmpx.so, the B200 (sm_100a) render-and-compare engine behind the MegaPose
+ * mpx.h -- C ABI of libmpx.so, the H100 (sm_90a) render-and-compare engine behind the MegaPose
  * inference API.  This is the drop-in boundary: plain pointers and sizes, no torch types.
  *
  * Conventions (all entry points):
@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define MPX_ABI_VERSION 4
+#define MPX_ABI_VERSION 5
 
 /* ---- library ------------------------------------------------------------------------------ */
 int mpx_abi_version(void);
@@ -208,11 +208,11 @@ size_t mpx_net_input_bytes(int n, int h, int w, int c_pad);
 /* single convolution (also the unit the parity tests exercise):
  *   d_x [n,H,W,C_in] act16, d_w [C_out, R*S*C_in] act16, d_bias [C_out] fp32,
  *   d_residual / d_out [n,P,Q,C_out] act16 (residual may be NULL)
- *   relu: bit 0 = ReLU; bit 1 = the weights are the space-to-depth form of the 7x7 stem (4x4 taps over C_in = 64: the 15 of
- *   64 (tap, 16-channel) slices that are zero by construction are not multiplied, megapose6d_b200/backbone.py: _stem_s2d);
+ *   relu: bit 0 = ReLU; bit 1 = the weights are the space-to-depth form of the 7x7 stem (4x4 taps over C_in = 64,
+ *   megapose6d_b200/backbone.py: _stem_s2d; 15 of its 64 (tap, 16-channel) slices are zero by construction);
  *   bit 2 = fused 3x3/s2/p1 max-pool (models/torchvision_resnet.py:197 `self.maxpool` right after the stem's ReLU): d_out is
- *   then the ZEROED [n, (P-1)/2+1, (Q-1)/2+1, C_out] tensor and is max-reduced into; needs bit 0, no residual, and returns
- *   MPX_ERR_UNSUPPORTED (nothing launched, no error text) for shapes the pair window kernel does not serve
+ *   then the ZEROED [n, (P-1)/2+1, (Q-1)/2+1, C_out] tensor and is max-reduced into; needs bit 0, no residual and
+ *   block_n = 0, and returns MPX_ERR_UNSUPPORTED (nothing launched, no error text) otherwise
  *   block_n: 0 = auto, else 64|128|256; max_ctas: 0 = one per SM */
 int mpx_conv2d(const void* d_x, int n, int h, int w, int c_in, const void* d_w,
                     const float* d_bias, int c_out, int r, int s, int stride, int pad_lo_h,
@@ -228,50 +228,16 @@ int mpx_conv2d_splitk(const void* d_x, int n, int h, int w, int c_in, const void
                            int pad_lo_w, int pad_hi_h, int pad_hi_w, int relu, const void* d_residual,
                            void* d_out, int block_n, int splits, void* stream);
 
-/* kernel selection bits for block_n == 0 (auto), default 60866571 = 1 + 2 + 8 + 16384 + 32768 + 2097152 + 8388608 + 16777216 + 33554432:
- *   1   window kernels: 64->64 stride-1 convolutions (stem, layer1) and 128->128 3x3 (layer2) load their activations
- *       once per tile as a contiguous window and address the filter taps as row-shifted operand descriptors
- *   2   the CTA-pair (cta_group::2) kernel serves 256-wide tiles;  4  and 128-wide tiles
- *   8   mpx_net_forward splits the K loop of layers 2-4 over a thread-block cluster for batches <= 64
- *   16  a single epilogue warp set in the 64->64 window kernel (default two)
- *   32  a single MMA-issuing thread in the 64->64 window kernel (default two);  64  three
- *   128 three epilogue warp sets
- *   256 disable the single-CTA layer2 window kernel (TMA-im2col kernel instead)
- *   512 launch without programmatic dependent launch;  1024 older row-group choice of the window kernel (diagnostic)
- *   16384 the layer2 window kernel on CTA pairs (cta_group::2, two MMA issuers in the leader): layer2 0.167 -> 0.153 ms
- *   32768 the 64 -> 64 window kernel (stem, layer1) on CTA pairs: layer1 0.255 -> 0.227 ms per convolution at batch 576
- *   131072 do not skip the structurally zero K slices of the space-to-depth stem weights (diagnostic)
- *   262144 / 524288 cap the automatic small-batch K split (bit 8) at 2 / 1 CTAs per tile: less SM time per layer at a higher
+/* convolution options, default 8.  One kernel serves every shape (TMA im2col + wgmma, 128-row tiles, 64/128/256-wide
+ * tiles chosen from the shape); the bits choose how the network drives it:
+ *   8   mpx_net_forward splits the K loop of the convolutions after the stem over a thread-block cluster for batches <= 64
+ *   512 launch without programmatic dependent launch
+ *   262144 / 524288 cap the automatic small-batch K split (bit 3) at 2 / 1 CTAs per tile: less SM time per layer at a higher
  *       latency (set before graphs are captured; the trade for two frames in flight, frame_pipeline.py)
- *   1048576 row-per-thread epilogue in the 64 -> 64 pair window kernel (round-1 form; default: staged, coalesced)
- *   2097152 mpx_net_forward lets the stem's pair window kernel max-pool in its epilogue (mpx_conv2d relu bit 2): the
- *       full-resolution stem output is never stored; network forward at batch 576: 6.51 -> 6.14 ms
- *   8388608 the 64 -> 64 pair window kernel slides its activation window: every CTA owns a contiguous run of 128-row blocks,
- *       the activations live in a ring of 16 KB chunks (one new chunk per block instead of a whole window: L2 -> SM reads 4x
- *       lower on the stem) and the residual rows arrive by TMA in the layout of the staging tiles: layer1 conv2 + residual
- *       0.246 -> 0.195 ms, bit-identical outputs; runs shorter than 8 blocks per CTA keep the reloading kernel (bit 15)
- *   16777216 the layer2 pair window kernel stages its epilogue through shared memory: residual rows by TMA into 128B-swizzled
- *       tiles, overwritten in place, stored as whole 128-byte lines (the weight ring gives up 3 of 12 stages for the 64 KB):
- *       layer2 conv2 + residual 0.190 -> 0.163 ms, bit-identical outputs
- *   33554432 the same for the 256-wide CTA-pair im2col kernel (layers 3-4), one 128-channel half of the tile at a time through a
- *       32 KB staging tile, bias read from global memory; only for K >= 768 (the 1x1 downsamples keep the row form):
- *       layer3 conv2 + residual 0.151 -> 0.147 ms, bit-identical outputs
- * (r02 A/B, profiles/r02_layer_table_mode_bits.json; the other round-1 candidates -- pair-window kernels for layer3/4 and
- * 128-wide layer2 tiles, residual preload -- measured no gain and were removed.)
- * 0 = single-CTA TMA-im2col kernel only */
+ *   2097152 mpx_net_forward lets the stem's epilogue max-pool (mpx_conv2d relu bit 2) instead of storing the stem output and
+ *       running mpx_maxpool3x3s2 on it; the outputs are identical
+ * Other bits are accepted and have no effect. */
 int mpx_conv_set_mode(int mode);
-
-/* bring-up probe (tools/gpu_probe_rowshift.py): D[128,64] = A[r0:r0+128, :64] * B[64,64]^T with the UMMA
- * A descriptor started r0 rows into a TMA-written 128B-swizzled tile; d_a [144,64] act16, d_b [64,64] act16 */
-int mpx_debug_umma_rowshift(const void* d_a, const void* d_b, int r0, int base_offset, float* d_out,
-                            void* stream);
-
-/* measurement probe (tools/gpu_mma_probe.py): mean cycles per tcgen05.mma of shape (128 * cta_group) x n x 16, operands in
- * shared memory, with `chains` (1|2|4) independent accumulators interleaved by each of `issuers` (1..4) issuing threads (one
- * per warp); *h_cycles_per_mma = SM time per MMA, *h_issue_cycles_per_mma (may be NULL) = one thread's time per instruction
- * issued, before the commit; synchronous */
-int mpx_debug_mma_probe(int cta_group, int n, int chains, int issuers, int n_mma, double* h_cycles_per_mma,
-                        double* h_issue_cycles_per_mma);
 
 /* 3x3/s2/p1 max pool, act16 NHWC (torchvision_resnet.py:302) */
 int mpx_maxpool3x3s2(const void* d_x, int n, int h, int w, int c, void* d_out, void* stream);

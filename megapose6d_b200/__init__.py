@@ -1,4 +1,4 @@
-"""B200-native render-and-compare pose engine with the MegaPose inference API.
+"""H100-native render-and-compare pose engine with the MegaPose inference API.
 
 Public surface (mirrors the reference's import points):
     PoseEstimator, PosePredictor, BatchRenderer (alias Panda3dBatchRenderer), ObservationTensor,

@@ -14,7 +14,7 @@ import torch
 
 _LIB_PATH = Path(__file__).resolve().parent / "csrc" / "libmpx.so"
 _lib: Optional[ctypes.CDLL] = None
-ABI_VERSION = 4  # MPX_ABI_VERSION of include/mpx.h this binding was written against
+ABI_VERSION = 5  # MPX_ABI_VERSION of include/mpx.h this binding was written against
 
 
 class MpxError(RuntimeError):
@@ -40,8 +40,6 @@ def _declare(lib: ctypes.CDLL) -> None:
                                             c_int, c_int, vp, vp, c_size_t, vp]
     lib.mpx_render_crop_fused.argtypes = [vp, vp, vp, vp, c_int, c_int, c_int, c_uint32, vp, c_int, c_int, c_int, vp,
                                           vp, c_int, vp, c_int, c_int, vp, vp, c_size_t, vp]
-    lib.mpx_debug_mma_probe.argtypes = [c_int, c_int, c_int, c_int, c_int, POINTER(ctypes.c_double), POINTER(ctypes.c_double)]
-    lib.mpx_debug_umma_rowshift.argtypes = [vp, vp, c_int, c_int, vp, vp]
     lib.mpx_pose_init_autodepth.argtypes = [vp, c_int, vp, vp, vp, vp, c_int, vp, vp]
     lib.mpx_normalize_T.argtypes = [vp, c_int, vp, vp]
     lib.mpx_crop_geometry.argtypes = [vp, c_int, vp, vp, vp, vp, c_int, c_float, c_int, c_int, c_int, c_int,
@@ -88,7 +86,7 @@ EXPORTS = [
     "mpx_raster_workspace_bytes", "mpx_raster_set_mode", "mpx_raster_render", "mpx_raster_render_fused", "mpx_render_crop_fused",
     "mpx_pose_init_autodepth", "mpx_normalize_T", "mpx_crop_geometry", "mpx_multiview_cameras",
     "mpx_pose_update", "mpx_topk_per_group", "mpx_image_to_nhwc4", "mpx_roi_align", "mpx_roi_align_fused",
-    "mpx_net_input_bytes", "mpx_conv2d", "mpx_conv2d_splitk", "mpx_conv_set_mode", "mpx_debug_umma_rowshift", "mpx_debug_mma_probe", "mpx_maxpool3x3s2", "mpx_avgpool_linear",
+    "mpx_net_input_bytes", "mpx_conv2d", "mpx_conv2d_splitk", "mpx_conv_set_mode", "mpx_maxpool3x3s2", "mpx_avgpool_linear",
     "mpx_net_create", "mpx_net_create_preact", "mpx_net_destroy", "mpx_net_set_graphs", "mpx_net_workspace_bytes", "mpx_net_forward",
 ]
 

@@ -4,7 +4,7 @@ Takes the parameters of the reference's `vanilla_resnet34` backbone
 (src/megapose/models/torchvision_resnet.py:181-316, created by
 training/pose_models_cfg.py:106-109 with `num_classes=512, n_input_channels=C`) and of the head
 (`pose_fc` or `views_logits_head`, models/pose_rigid.py:120-130) in the reference's state-dict
-layout and repacks them once for the tcgen05 kernels:
+layout and repacks them once for the wgmma kernels:
   * eval-mode BatchNorm folded into the preceding conv (w' = w*g/sqrt(var+eps), b' = beta - mean*g/sqrt(var+eps));
   * conv weights OIHW fp32 -> [C_out, R*S*C_in] in the library's 16-bit type (`_abi.act_dtype()`: fp16 unless the
     library was built for bf16), K ordered (r, s, c);

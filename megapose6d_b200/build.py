@@ -1,8 +1,8 @@
-"""Build libmpx.so (the C-ABI CUDA library) in-tree for sm_100a.
+"""Build libmpx.so (the C-ABI CUDA library) in-tree for sm_90a (H100).
 
 `python -m megapose6d_b200.build` or `build_library()`; nvcc cross-compiles without a GPU.
-The shared object lands next to the sources (megapose6d_b200/csrc/libmpx.so) so that it travels
-with the repository snapshot to the GPU box.
+The shared object lands next to the sources (megapose6d_b200/csrc/libmpx.so), where the package loads it
+from the source tree.
 """
 from __future__ import annotations
 
@@ -15,9 +15,10 @@ from pathlib import Path
 
 CSRC = Path(__file__).resolve().parent / "csrc"
 LIB_PATH = CSRC / "libmpx.so"
-SOURCES = ["abi.cu", "conv_tc.cu", "net.cu", "raster.cu", "geom.cu", "crop.cu"]
+SOURCES = ["abi.cu", "conv_wgmma.cu", "net.cu", "raster.cu", "geom.cu", "crop.cu"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *ARCH_FLAGS,
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -64,7 +65,7 @@ def build_library(force: bool = False, verbose: bool = False) -> Path:
 
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB_PATH),
+    link = [nvcc, "-shared", *ARCH_FLAGS, "-o", str(LIB_PATH),
             *map(str, objs), "-Xcompiler", "-fPIC", "-cudart", "static"]
     res = subprocess.run(link, capture_output=True, text=True)
     if res.returncode != 0:

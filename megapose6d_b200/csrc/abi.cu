@@ -341,19 +341,6 @@ int mpx_conv2d_splitk(const void* d_x, int n, int h, int w, int c_in, const void
                       splits == 0 ? -1 : splits);
 }
 
-int mpx_debug_mma_probe(int cta_group, int n, int chains, int issuers, int n_mma, double* h_cycles_per_mma,
-                        double* h_issue_cycles_per_mma) {
-  MPX_NOT_NULL(h_cycles_per_mma);
-  return mma_probe(cta_group, n, chains, issuers, n_mma, h_cycles_per_mma, h_issue_cycles_per_mma);
-}
-
-int mpx_debug_umma_rowshift(const void* d_a, const void* d_b, int r0, int base_offset, float* d_out, void* stream) {
-  MPX_NOT_NULL(d_a);
-  MPX_NOT_NULL(d_b);
-  MPX_NOT_NULL(d_out);
-  return umma_rowshift_probe(d_a, d_b, r0, base_offset, d_out, static_cast<cudaStream_t>(stream));
-}
-
 int mpx_maxpool3x3s2(const void* d_x, int n, int h, int w, int c, void* d_out, void* stream) {
   MPX_NOT_NULL(d_x);
   MPX_NOT_NULL(d_out);

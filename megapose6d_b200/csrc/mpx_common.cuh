@@ -1,4 +1,4 @@
-// Shared device/host helpers for the mpx kernels (sm_100a only).
+// Shared device/host helpers for the mpx kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -47,7 +47,7 @@ inline int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return (g_sm_limit > 0 && g_sm_limit < n) ? g_sm_limit : n;
 }
@@ -77,7 +77,7 @@ __device__ __forceinline__ float warp_sum(float v) {
 
 // ---------------------------------------------------------------------------------------------
 // 16-bit storage type of weights and activations ("act").  fp16 by default: the tensor core runs fp16 and bf16 operands
-// at the same rate (tcgen05 kind::f16, fp32 accumulation either way), fp16 carries three more mantissa bits, and fp16 is
+// at the same rate (wgmma .f16 / .bf16, fp32 accumulation either way), fp16 carries three more mantissa bits, and fp16 is
 // what the reference's networks were trained under (torch.cuda.amp.autocast, training/train_megapose.py:299).  The
 // narrower range is handled by a saturating conversion (values beyond +-65504 clamp instead of becoming inf).
 // -DMPX_ACT_BF16 selects bf16 (same kernels; diagnostic A/B of the two number formats).
@@ -86,7 +86,6 @@ __device__ __forceinline__ float warp_sum(float v) {
 typedef __nv_bfloat16 act_t;
 typedef __nv_bfloat162 act_t2;
 constexpr int kActIsFp16 = 0;
-constexpr uint32_t kIdescAB = (1u << 7) | (1u << 10);  // InstrDescriptor a_format / b_format = BF16
 __device__ __forceinline__ uint32_t pack_act2(float lo, float hi) {
   act_t2 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
@@ -100,7 +99,6 @@ __device__ __forceinline__ act_t to_act(float v) { return __float2bfloat16_rn(v)
 typedef __half act_t;
 typedef __half2 act_t2;
 constexpr int kActIsFp16 = 1;
-constexpr uint32_t kIdescAB = 0u;                      // InstrDescriptor a_format / b_format = F16
 __device__ __forceinline__ uint32_t pack_act2(float lo, float hi) {
   uint32_t r;  // cvt packs its first source into the upper half
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
@@ -130,7 +128,7 @@ __device__ __forceinline__ float depth_norm(float d, float z, int kind) {
 // Programmatic dependent launch (PDL): a kernel launched through launch_pdl may start while its stream predecessor is
 // still running, as soon as every CTA of the predecessor has executed pdl_trigger() (or exited).  It must call pdl_wait()
 // before it touches memory the predecessor writes (or writes memory the predecessor reads); everything before that --
-// barrier / TMEM set-up, descriptor prefetch, constant loads -- overlaps with the predecessor's tail.  The chains of
+// barrier set-up, descriptor prefetch, constant loads -- overlaps with the predecessor's tail.  The chains of
 // small-batch kernels (36 convolutions of ~6-10 us each per network forward) are bound by exactly that fixed cost.
 // Without a PDL-aware predecessor both calls are no-ops.  mpx_conv_set_mode bit 9 (512) launches without the attribute.
 // ---------------------------------------------------------------------------------------------
@@ -165,7 +163,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 }
 
 // ---------------------------------------------------------------------------------------------
-// cross-file declarations (conv_tc.cu, net.cu)
+// cross-file declarations (conv_wgmma.cu, net.cu)
 // ---------------------------------------------------------------------------------------------
 extern long long g_launches;  // kernels launched by this library (host-side counter)
 void conv_profile_enable(int on);
@@ -180,7 +178,7 @@ struct ConvDesc {
   int C_out, R, S, stride;
   int pad_lo_h, pad_lo_w, pad_hi_h, pad_hi_w;
   int relu;
-  int s2d_stem;  // 1: the weights are the space-to-depth form of the 7x7 stem (zero slices are skipped), see conv_tc.cu
+  int s2d_stem;  // 1: the weights are the space-to-depth form of the 7x7 stem (megapose6d_b200/backbone.py: _stem_s2d)
   int pool;      // 1: `out` is the ZERO-INITIALISED [n, (H-1)/2+1, (W-1)/2+1, C_out] tensor and receives the 3x3/s2/p1 max-pool of
                  //    the (ReLU'd) result through vector max-reductions; conv_forward returns MPX_ERR_UNSUPPORTED (no error set)
                  //    when no kernel with that epilogue serves the shape
@@ -190,8 +188,6 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
                  const void* residual, void* out, int block_n_override, int max_ctas,
                  cudaStream_t stream, int splitk = 0);
 int conv_out_dim(int in, int pad_lo, int pad_hi, int k, int stride);
-int mma_probe(int cta_group, int n, int chains, int issuers, int n_mma, double* cycles_per_mma, double* issue_cycles_per_mma);
-int umma_rowshift_probe(const void* a, const void* b, int r0, int base_off, float* out, cudaStream_t stream);
 int maxpool3x3s2(const void* x, int n, int h, int w, int c, void* out, cudaStream_t stream);
 int avgpool_linear(const void* x, int n, int hw, int c, const float* w, const float* b, int out_dim,
                    float* out, cudaStream_t stream);

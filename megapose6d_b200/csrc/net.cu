@@ -1,4 +1,4 @@
-// ResNet-34 execution plan around the tcgen05 convolution: max-pool, pooled linear tail, and the
+// ResNet-34 execution plan around the wgmma convolution: max-pool, pooled linear tail, and the
 // fixed 36-convolution schedule of the reference backbone
 // (reference: src/megapose/models/torchvision_resnet.py:74-120 BasicBlock, :298-311 forward order;
 //  heads: src/megapose/models/pose_rigid.py:120-130, 314-334).
@@ -350,7 +350,7 @@ int net_forward(const Net* cnet, const void* x, int n, int h, int w, float* out,
   return MPX_OK;
 }
 
-// Stem convolution + ReLU followed by the 3x3/s2/p1 max-pool.  With mode bit 21 (2097152) the pair window kernel pools in its
+// Stem convolution + ReLU followed by the 3x3/s2/p1 max-pool.  With mode bit 21 (2097152) the convolution pools in its
 // epilogue (max-reductions into the zeroed pooled tensor): the full-resolution stem output -- 2.46 MB per sample at 240x320,
 // written once and read once by nothing but the pool -- never exists.  Falls back to the two kernels when the shape is not
 // served (the memset is then wasted, nothing else).

@@ -1,4 +1,4 @@
-// Batched software rasteriser for sm_100a: one persistent CTA per view.
+// Batched software rasteriser for sm_90a: one persistent CTA per view.
 //
 // Replaces the Panda3D/OpenGL path of the reference renderer
 // (reference: src/megapose/panda3d_renderer/panda3d_batch_renderer.py:217-282 render,

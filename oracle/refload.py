@@ -1,9 +1,9 @@
-"""oracle/refload.py -- run the REAL reference code from /root/reference by file path.
+"""oracle/refload.py -- run the REAL reference code by file path.
 
-TEST INFRASTRUCTURE ONLY, and only usable where /root/reference exists (this container; never the
-GPU box).  Purpose: (1) validate oracle/{lib3d_ref,resnet_ref,pipeline_ref}.py against the
-reference's own functions, (2) generate the golden fixtures in tests/golden/ (script:
-tools/make_golden.py).
+TEST INFRASTRUCTURE ONLY, and only usable where a checkout of the reference (github.com/megapose6d/megapose6d) is named by
+$MEGAPOSE_REFERENCE.  Purpose: record what the reference returns, as the golden fixtures in tests/golden/
+(tools/make_golden.py; tests/golden/reference/ with MPX_RECORD_REFERENCE=1, see tests/helpers.py: reference_outputs),
+against which the oracle and the product are checked.
 
 `import megapose` fails here (pinocchio, omegaconf, roma, panda3d, ... are absent and the package
 __init__ needs env vars, SURVEY.md 8c), so the reference files on the hot path are loaded with
@@ -20,6 +20,7 @@ from __future__ import annotations
 
 import importlib.util
 import logging
+import os
 import sys
 import time
 import types
@@ -28,13 +29,14 @@ from pathlib import Path
 import numpy as np
 import torch
 
-REF_ROOT = Path("/root/reference/src/megapose")
+# the reference's package directory, or None when no checkout is named
+REF_ROOT = Path(os.environ["MEGAPOSE_REFERENCE"]).resolve() / "src" / "megapose" if os.environ.get("MEGAPOSE_REFERENCE") else None
 
 _loaded = None
 
 
 def available() -> bool:
-    return REF_ROOT.is_dir()
+    return REF_ROOT is not None and REF_ROOT.is_dir()
 
 
 def _pkg(name: str) -> types.ModuleType:
@@ -73,7 +75,7 @@ def load():
     if _loaded is not None:
         return _loaded
     if not available():
-        raise RuntimeError("/root/reference is not present on this machine")
+        raise RuntimeError(f"no reference source at {REF_ROOT}: set MEGAPOSE_REFERENCE to a checkout of the reference")
     from . import lib3d_ref
 
     for name in ["megapose", "megapose.lib3d", "megapose.models", "megapose.utils", "megapose.inference",

@@ -1,5 +1,6 @@
-"""Detector front-end (SURVEY 8 f4): the product's Detector against the reference's own class loaded by path
-(src/megapose/inference/detector.py:34-142), fed by the same stand-in network; load_detector round trip."""
+"""Detector front-end (SURVEY 8 f4): the product's Detector against what the reference's own class
+(src/megapose/inference/detector.py:34-142, loaded by path to record tests/golden/reference/detector_*.npz) returned for the
+same stand-in network; load_detector round trip."""
 import importlib.util
 import sys
 import types
@@ -12,6 +13,7 @@ from megapose6d_b200 import detector as D
 from megapose6d_b200.load_model import Cfg
 from megapose6d_b200.types import ObservationTensor
 from oracle import refload
+from tests import helpers
 
 
 class FakeMaskRCNN(torch.nn.Module):
@@ -47,6 +49,7 @@ def _reference_detector_cls():
 
 
 def _same(a, b):
+    """a: the product's detections, b: the reference's (a collection stored with helpers.collection_arrays)."""
     da, db = a.infos.reset_index(drop=True), b.infos.reset_index(drop=True)
     # the pandas of this image drops the grouping columns inside the reference's groupby().apply() (add_instance_id,
     # inference/utils.py:166-169; the reference's pinned pandas keeps them): compare the columns the reference still has
@@ -58,27 +61,35 @@ def _same(a, b):
         else:
             assert list(da[c]) == list(db[c]), c
     assert torch.equal(a.bboxes.cpu(), b.bboxes.cpu()) and a.bboxes.dtype == b.bboxes.dtype
-    ta, tb = set(a._tensors.keys()), set(b._tensors.keys())
+    ta, tb = set(a.tensors.keys()), set(b.tensors.keys())
     assert ta == tb
     if "masks" in ta:
         assert torch.equal(a.masks.cpu(), b.masks.cpu())
 
 
-@pytest.mark.skipif(not refload.available(), reason="needs /root/reference")
+KWARGS = [dict(), dict(detection_th=0.4), dict(output_masks=True, mask_th=0.6),
+          dict(one_instance_per_class=True, detection_th=0.1, output_masks=True)]
+
+
 @pytest.mark.parametrize("counts", [(3, 0, 5), (1,), (4, 4)])
-@pytest.mark.parametrize("kw", [dict(), dict(detection_th=0.4), dict(output_masks=True, mask_th=0.6),
-                                dict(one_instance_per_class=True, detection_th=0.1, output_masks=True)])
+@pytest.mark.parametrize("kw", KWARGS)
 def test_detector_matches_reference_class(counts, kw):
-    RefDetector, ref = _reference_detector_cls()
-    images = torch.rand(len(counts), 3, 24, 32)
+    images = torch.rand(len(counts), 3, 24, 32, generator=torch.Generator().manual_seed(len(counts)))
     K = torch.eye(3).repeat(len(counts), 1, 1)
+    rgb = (np.random.RandomState(0).rand(24, 32, 3) * 255).astype(np.uint8)
+
+    def reference():
+        RefDetector, ref = _reference_detector_cls()
+        with refload.cpu_cuda_patch():
+            want = RefDetector(FakeMaskRCNN(counts)).get_detections(ref.types.ObservationTensor(images, K), **kw)
+        return dict(**helpers.collection_arrays("detections", want),
+                    image_tensor=RefDetector(FakeMaskRCNN(counts)).image_tensor_from_numpy(rgb))
+
+    stored = helpers.reference_outputs(f"detector_{'_'.join(map(str, counts))}_kw{KWARGS.index(kw)}", reference)
     mine = D.Detector(FakeMaskRCNN(counts))
     got = mine.get_detections(ObservationTensor(images, K), **kw)
-    with refload.cpu_cuda_patch():
-        want = RefDetector(FakeMaskRCNN(counts)).get_detections(ref.types.ObservationTensor(images, K), **kw)
-    _same(got, want)
-    rgb = (np.random.RandomState(0).rand(24, 32, 3) * 255).astype(np.uint8)
-    assert torch.equal(mine.image_tensor_from_numpy(rgb), RefDetector(FakeMaskRCNN(counts)).image_tensor_from_numpy(rgb))
+    _same(got, helpers.StoredCollection(stored, "detections"))
+    assert torch.equal(mine.image_tensor_from_numpy(rgb), stored["image_tensor"])
 
 
 def test_detector_without_detections():

@@ -179,7 +179,7 @@ def test_raster_big_batch_low_poly_and_odd_size(big_batch_mode):
     ds = RigidObjectDataset([RigidObject("box", mesh=procedural.textured_box(seed=1)),
                              RigidObject("ball", mesh=procedural.bumpy_sphere(n_seg=40, n_lat=21))])
     rm = helpers.ref_meshes_from_dataset(ds)
-    n = 2 * 148 + 5
+    n = 2 * _abi.lib().mpx_sm_count() + 5
     labels = [ds[i % 2].label for i in range(n)]
     TCO = _poses(n, 9, z_range=(0.2, 0.6))
     Kc = torch.tensor([[420.0, 0, 75], [0, 420, 50], [0, 0, 1]]).repeat(n, 1, 1)
@@ -235,7 +235,7 @@ def test_raster_empty_batch():
 def test_raster_many_views_persistent_loop(scene):
     """More views than resident CTAs: one view per CTA, persistent loop over the rest (no row strips)."""
     ds, images, K, db, rm = scene
-    n = 2 * 148 * 2 + 37
+    n = 2 * _abi.lib().mpx_sm_count() * 2 + 37
     labels = [ds[i % 3].label for i in range(n)]
     TCO = _poses(n, 77, z_range=(0.3, 0.9))
     Kc = torch.tensor([[400.0, 0, 40], [0, 400, 32], [0, 0, 1]]).repeat(n, 1, 1)
@@ -297,7 +297,7 @@ def test_textured_meshes_many_views_and_fused_input():
     """The one-kernel path (more views than CTA slots) with textures, and the fused network-input form."""
     ds = _textured_ds()
     rm = helpers.ref_meshes_from_dataset(ds)
-    n = 2 * 148 + 19
+    n = 2 * _abi.lib().mpx_sm_count() + 19
     labels = [ds[i % 3].label for i in range(n)]
     TCO = _poses(n, 34, z_range=(0.25, 0.6))
     Kc = torch.tensor([[300.0, 0, 40], [0, 300, 32], [0, 0, 1]]).repeat(n, 1, 1)

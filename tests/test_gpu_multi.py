@@ -85,9 +85,9 @@ def test_two_rank_pipeline_equals_single_rank():
     assert torch.equal(results[0]["coarse"], results[1]["coarse"])
     assert results[0]["hyp"] == results[1]["hyp"]
     assert torch.equal(results[0]["poses"], results[1]["poses"])
-    # against the single-rank run the per-rank batch sizes differ, and with them the convolution kernels that are selected
-    # (split-K for small batches, window kernels for large ones): same products, different fp32 summation order, so the
-    # bf16 network outputs agree to rounding, not bit for bit
+    # against the single-rank run the per-rank batch sizes differ, and with them the tile widths and K splits of the
+    # convolutions: same products, different fp32 summation order, so the 16-bit network outputs agree to rounding, not
+    # bit for bit
     d = (results[0]["coarse"] - single["coarse"]).abs()
     print("two-rank vs single-rank coarse logits: max |d| = %.4g, mean |d| = %.4g" % (d.max(), d.mean()))
     assert d.max() <= 0.1 and d.mean() <= 0.02

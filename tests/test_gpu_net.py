@@ -1,4 +1,8 @@
-"""GPU parity of the tcgen05 convolution and of the whole ResNet-34 engine.
+"""GPU parity of the wgmma convolution and of the whole ResNet-34 engine.
+
+The kernel-selection values of mpx_conv_set_mode that chose between kernel variants (window kernels, CTA pairs, staged
+epilogues) are accepted and have no effect in this build: one kernel serves every shape.  The tests that run a shape under
+several of those values keep checking that the result does not depend on them, and each result against fp32 torch.
 
 Tolerances (stated, floating point):
   * single conv vs fp32 torch conv on the same 16-bit-rounded operands: |err| <= ULP * max|ref| + ATOL, one rounding
@@ -22,10 +26,9 @@ from tests import helpers
 pytestmark = pytest.mark.gpu
 ACT = _abi.act_dtype() if torch.cuda.is_available() else torch.float16
 ULP, ATOL = (2 ** -10, 2e-3) if ACT == torch.float16 else (2 ** -7, 1e-2)
-SINGLE_CTA_MODE = 11  # window | pair(256) | split-K, without the CTA-pair window kernels of bits 14 / 15
-DEFAULT_CONV_MODE = 60866571  # window | pair(256) | split-K in the network | CTA-pair window kernels (bits 14, 15) | fused max-pool
-# (bit 21) | sliding window in the 64 -> 64 pair kernel (bit 23) | staged epilogues in the layer2 (bit 24) and layer3-4 (bit 25) pair kernels
-RELOAD_MODE = DEFAULT_CONV_MODE & ~8388608  # without bit 23: conv_windowq_kernel (whole window reloaded per tile) everywhere
+SINGLE_CTA_MODE = 11  # kernel-variant bits 0, 1 and split-K in the network (bit 3)
+DEFAULT_CONV_MODE = 8  # the library's default (include/mpx.h): split-K in the network for small batches
+RELOAD_MODE = DEFAULT_CONV_MODE | 32768  # a kernel-variant bit: no effect
 
 
 def _conv_ref(x, w, bias, stride, pads, relu, residual):
@@ -187,7 +190,7 @@ def test_resnet34_engine_vs_oracle(cfg_name):
 
 
 WINDOW_CASES = [
-    # the 64 -> 64 stride-1 "same" convolutions are served by the shared-memory window kernel (mode bit 0)
+    # the 64 -> 64 stride-1 "same" convolutions of the stem and layer1, under mode bit 0 set and cleared
     ("win_3x3", 3, 60, 80, 3, 3, (1, 1, 1, 1), True, True),
     ("win_3x3_tiny", 5, 7, 9, 3, 3, (1, 1, 1, 1), False, False),
     ("win_stem", 2, 120, 160, 4, 4, (2, 2, 1, 1), True, False),
@@ -197,7 +200,7 @@ WINDOW_CASES = [
 
 @pytest.mark.parametrize("case", WINDOW_CASES, ids=[c[0] for c in WINDOW_CASES])
 def test_window_and_im2col_kernels_agree(case):
-    """Both kernels accumulate the same products in fp32 (possibly in a different order): outputs agree to one bf16 ulp,
+    """The same products accumulated in fp32 under either mode value: outputs agree to one 16-bit ulp,
     and each is within the stated tolerance of the fp32 reference."""
     name, n, h, w, r, s, pads, relu, use_res = case
     g = torch.Generator(device="cuda").manual_seed(7)
@@ -265,8 +268,8 @@ WIN2_CASES = [
 
 @pytest.mark.parametrize("case", WIN2_CASES, ids=[c[0] for c in WIN2_CASES])
 def test_layer2_window_kernel_agrees_with_im2col_and_torch(case):
-    """conv_window2_kernel (128 -> 128, 3x3: activations loaded once per 256-row super-tile, one weight pass for two
-    tiles, two MMA issuers) vs the im2col kernel (mode bit 8 = 256 disables it) and fp32 torch."""
+    """The layer2 shape (128 -> 128, 3x3) with few CTAs for many tiles (persistent loop), under mode bit 8 cleared and
+    set, vs fp32 torch."""
     name, n, h, w, relu, use_res, max_ctas = case
     g = torch.Generator(device="cuda").manual_seed(23)
     x = torch.randn(n, h, w, 128, device="cuda", generator=g).to(ACT)
@@ -275,7 +278,7 @@ def test_layer2_window_kernel_agrees_with_im2col_and_torch(case):
     res = torch.randn(n, h, w, 128, device="cuda", generator=g).to(ACT) if use_res else None
     outs = []
     try:
-        for mode in (SINGLE_CTA_MODE, SINGLE_CTA_MODE | 256):  # single-CTA layer2 window kernel vs TMA-im2col kernel
+        for mode in (SINGLE_CTA_MODE, SINGLE_CTA_MODE | 256):
             _abi.lib().mpx_conv_set_mode(mode)
             out = torch.full((n, h, w, 128), float("nan"), device="cuda", dtype=ACT)
             _abi.check(_abi.lib().mpx_conv2d(_abi.ptr(x), n, h, w, 128, _abi.ptr(wt.view(128, -1)), _abi.ptr(bias), 128, 3, 3,
@@ -289,7 +292,7 @@ def test_layer2_window_kernel_agrees_with_im2col_and_torch(case):
     tol = ULP * ref.abs().max().item() + ATOL
     assert not torch.isnan(outs[0]).any()
     assert (outs[0] - ref).abs().max() <= tol and (outs[1] - ref).abs().max() <= tol
-    # different K order (panel-major) than the im2col kernel: equal up to one bf16 rounding
+    # equal up to one 16-bit rounding
     assert (outs[0] - outs[1]).abs().max() <= ULP * ref.abs().max().item()
 
 
@@ -324,8 +327,8 @@ PAIR_CASES = [
 
 @pytest.mark.parametrize("case", PAIR_CASES, ids=[c[0] for c in PAIR_CASES])
 def test_cta_pair_kernel_vs_torch_and_single_cta(case):
-    """tcgen05.mma.cta_group::2 kernel (mode bit 1; bit 2 also routes 128-wide tiles through it) vs fp32 torch and vs
-    the single-CTA kernel."""
+    """The shapes of layers 3-4 under three kernel-variant values of the mode (bits 1, 2, 25) vs fp32 torch; the results
+    are bit-identical."""
     name, n, h, w, cin, cout, r, s, stride, pads, relu, use_res = case
     g = torch.Generator(device="cuda").manual_seed(11)
     x = torch.randn(n, h, w, cin, device="cuda", generator=g).to(ACT)
@@ -349,7 +352,7 @@ def test_cta_pair_kernel_vs_torch_and_single_cta(case):
     ref = _conv_ref(x, wt, bias, stride, pads, relu, res)
     tol = ULP * ref.abs().max().item() + ATOL
     assert (outs[0] - ref).abs().max() <= tol and (outs[1] - ref).abs().max() <= tol
-    assert torch.equal(outs[0], outs[1])  # same products, same K order, fp32 accumulation in TMEM
+    assert torch.equal(outs[0], outs[1])  # same products, same K order, fp32 accumulation
     assert torch.equal(outs[0], outs[2])  # staged epilogue (residual by TMA, bias from global memory): same arithmetic
 
 
@@ -446,8 +449,8 @@ def test_pair_window64_kernel(case):
 @pytest.mark.parametrize("mode", [DEFAULT_CONV_MODE, SINGLE_CTA_MODE], ids=["cta_pairs", "single_cta"])
 def test_stem_space_to_depth_skips_zero_slices(mode):
     """The 7x7 / stride-2 stem runs as a 4x4 convolution over the space-to-depth input; 15 of its 64 (tap, sub-pixel) weight
-    slices are zero by construction and are not multiplied (K = 784 instead of 1024).  Skipping them adds exact zeros less:
-    the output is bit-identical to the unskipped run and matches torch's 7x7 / stride-2 convolution."""
+    slices are zero by construction.  With or without the space-to-depth flag (relu bit 1) and mode bit 17 the output is
+    bit-identical, and it matches torch's 7x7 / stride-2 convolution."""
     from megapose6d_b200.backbone import _stem_s2d
 
     n, h, w, c, c_pad = 5, 96, 128, 9, 16
@@ -497,6 +500,7 @@ def test_wide_resnet_engine_vs_oracle(backbone_str):
 
 
 SEPARATE_POOL_MODE = DEFAULT_CONV_MODE & ~2097152  # without bit 21: stem output stored, max-pool as its own kernel
+FUSED_POOL_MODE = DEFAULT_CONV_MODE | 2097152  # bit 21: the stem's epilogue max-pools
 POOL_CASES = [
     # name, n, h, w, r, pads, max_ctas
     ("stem_4x4", 3, 120, 160, 4, (2, 2, 1, 1), 6),
@@ -510,9 +514,9 @@ POOL_CASES = [
 
 @pytest.mark.parametrize("case", POOL_CASES, ids=[c[0] for c in POOL_CASES])
 def test_fused_maxpool_epilogue_equals_conv_then_maxpool(case):
-    """mpx_conv2d with relu bit 2 (conv_windowq_kernel's pooled epilogue: 16-byte max-reductions into the zeroed pooled
-    tensor) against the stored convolution followed by mpx_maxpool3x3s2: the maximum is exact, so the two agree value for
-    value (torch.equal on floats: +0 == -0), for even and odd sizes, image borders and warp-tile borders."""
+    """mpx_conv2d with relu bit 2 (the pooled epilogue: vector max-reductions into the zeroed pooled tensor) against the
+    stored convolution followed by mpx_maxpool3x3s2: the maximum is exact, so the two agree value for value (torch.equal on
+    floats: +0 == -0), for even and odd sizes, image borders and tile borders."""
     name, n, h, w, r, pads, max_ctas = case
     g = torch.Generator(device="cuda").manual_seed(43)
     x = torch.randn(n, h, w, 64, device="cuda", generator=g).to(ACT)
@@ -543,7 +547,7 @@ def test_fused_maxpool_epilogue_equals_conv_then_maxpool(case):
 
 @pytest.mark.parametrize("cfg_name,n", [("coarse", 7), ("refiner", 1)])
 def test_network_with_fused_maxpool_equals_unfused(cfg_name, n):
-    """The whole forward with mode bit 21 (stem epilogue pools; the default) against the stem followed by the max-pool kernel:
+    """The whole forward with mode bit 21 (the stem's epilogue pools) against the stem followed by the max-pool kernel:
     every later layer sees the same pooled tensor, so the outputs are identical."""
     cfg = dict(coarse=helpers.COARSE_CFG, refiner=helpers.REFINER_CFG)[cfg_name]
     sd = helpers.make_state_dict(cfg, seed=3)
@@ -551,7 +555,7 @@ def test_network_with_fused_maxpool_equals_unfused(cfg_name, n):
     x = helpers._calibration_batch(c, 42, n=n).cuda()
     outs = []
     try:
-        for mode in (SEPARATE_POOL_MODE, DEFAULT_CONV_MODE, DEFAULT_CONV_MODE):
+        for mode in (SEPARATE_POOL_MODE, FUSED_POOL_MODE, FUSED_POOL_MODE):
             _abi.lib().mpx_conv_set_mode(mode)
             eng = ResNet34Engine(sd, n_inputs=c, head=resnet_ref.head_name(sd))
             outs.append(eng(x).clone())  # first sight of a shape runs eagerly

@@ -27,7 +27,7 @@ def test_abi_library_loads_and_exports_every_declared_symbol():
     missing = [name for name in sorted(declared) if not hasattr(lib, name)]
     assert not missing, f"symbols declared in include/mpx.h but not exported: {missing}"
     assert set(_abi.EXPORTS) == declared
-    assert _abi.lib().mpx_abi_version() == _abi.ABI_VERSION == 4
+    assert _abi.lib().mpx_abi_version() == _abi.ABI_VERSION == 5
     assert _abi.lib().mpx_act_dtype() in (0, 1)
 
 

@@ -1,9 +1,12 @@
-"""Frame-level caller (megapose6d_b200/prediction_runner.py): host logic on the CPU with a stand-in estimator, the REAL
-reference caller (loaded by path, marker `reference`) as the checker, and a world_size-2 gloo run of the frame sharding.
+"""Frame-level caller (megapose6d_b200/prediction_runner.py): host logic on the CPU with a stand-in estimator, what the
+REAL reference caller returned as the checker (stored under tests/golden/reference/; the reference, loaded by path, runs only
+to re-record it), and a world_size-2 gloo run of the frame sharding.
 
 The stand-in estimator is a deterministic function of the observation and the detections; it works with the reference's
 collections and with ours, so the reference's `PredictionRunner` and ours can be driven by the same object."""
+import functools
 import importlib.util
+import json
 import os
 import pickle
 import socket
@@ -20,6 +23,7 @@ import torch.multiprocessing as mp
 from megapose6d_b200 import prediction_runner as pr
 from megapose6d_b200.example import CameraData, ObjectData
 from megapose6d_b200.types import InferenceConfig
+from tests import helpers
 
 
 # ------------------------------------------------------------------------------------------------------ fixtures
@@ -103,8 +107,8 @@ def _same_collection(a, b, drop=("time",)):
 
 
 # ------------------------------------------------------------------------------------------- the reference's caller
-@pytest.fixture(scope="module")
-def ref_caller():
+@functools.lru_cache(maxsize=None)
+def _ref_caller():
     """The reference's samplers.py, scene_dataset.py and prediction_runner.py, loaded by path on top of oracle/refload.py.
     Stubbed (absent packages): webdataset, pinocchio's Transform (a numpy 4x4 holder: the runner only reads `.matrix`),
     megapose.utils.random (its two pure-Python helpers are exec'ed from the source), DataLoader workers (n_workers=0)."""
@@ -170,109 +174,149 @@ def _to_reference_observation(ref_caller, obs):
                               object_datas=objs, camera_data=cam)
 
 
-@pytest.mark.reference
-def test_sampler_matches_the_reference(ref_caller):
+SAMPLER_CASES = [(n, world, shuffle, rank) for n in (1, 2, 7, 50, 1000) for world in (1, 2, 3, 8) for shuffle in (True, False)
+                 for rank in range(world)]
+
+
+def test_sampler_matches_the_reference():
+    def reference():
+        S = _ref_caller().samplers.DistributedSceneSampler
+        out = {}
+        for n, world, shuffle, rank in SAMPLER_CASES:
+            a = S(range(n), world, rank, shuffle=shuffle)
+            out[f"{n}/{world}/{shuffle}/{rank}"] = np.asarray(list(a), dtype=np.int64)
+            out[f"{n}/{world}/{shuffle}/{rank}/len"] = len(a)
+        return out
+
+    want = helpers.reference_outputs("distributed_scene_sampler", reference)
     state = np.random.get_state()[1].copy()
-    for n in (1, 2, 7, 50, 1000):
-        for world in (1, 2, 3, 8):
-            for shuffle in (True, False):
-                for rank in range(world):
-                    a = ref_caller.samplers.DistributedSceneSampler(range(n), world, rank, shuffle=shuffle)
-                    b = pr.DistributedSceneSampler(range(n), world, rank, shuffle=shuffle)
-                    assert list(a) == list(b) and len(a) == len(b)
+    for n, world, shuffle, rank in SAMPLER_CASES:
+        b = pr.DistributedSceneSampler(range(n), world, rank, shuffle=shuffle)
+        key = f"{n}/{world}/{shuffle}/{rank}"
+        assert want[key].tolist() == list(b) and int(want[key + "/len"]) == len(b)
     assert np.array_equal(state, np.random.get_state()[1])
 
 
-@pytest.mark.reference
 @pytest.mark.parametrize("with_init", [False, True])
-def test_collate_matches_the_reference(ref_caller, with_init):
+def test_collate_matches_the_reference(with_init):
     obs = make_observations(3, with_init=with_init)
-    for labels in (None, ["obj_000001", "obj_000002", "obj_000003"]):
-        a = ref_caller.scene_dataset.SceneObservation.collate_fn([_to_reference_observation(ref_caller, o) for o in obs], labels)
+    label_sets = (None, ["obj_000001", "obj_000002", "obj_000003"])
+
+    def reference():
+        R = _ref_caller()
+        out = {}
+        for i, labels in enumerate(label_sets):
+            a = R.scene_dataset.SceneObservation.collate_fn([_to_reference_observation(R, o) for o in obs], labels)
+            out.update({f"{i}/keys": helpers.json_array(sorted(a)), f"{i}/rgb": a["rgb"], f"{i}/depth": a["depth"],
+                        f"{i}/im_infos": helpers.json_array(a["im_infos"]), f"{i}/K": a["cameras"].K})
+            for k in ("gt_detections", "gt_data", "initial_data"):
+                out[f"{i}/{k}/is_none"] = a[k] is None
+                if a[k] is not None:
+                    out.update(helpers.collection_arrays(f"{i}/{k}", a[k]))
+        return out
+
+    want = helpers.reference_outputs(f"collate_init{int(with_init)}", reference)
+    for i, labels in enumerate(label_sets):
         b = pr.SceneObservation.collate_fn(obs, labels)
-        assert set(a) == set(b)
-        assert torch.equal(a["rgb"], b["rgb"]) and torch.equal(a["depth"], b["depth"])
-        assert a["im_infos"] == b["im_infos"]
-        assert torch.equal(a["cameras"].K, b["cameras"].K)
+        assert json.loads(str(want[f"{i}/keys"])) == sorted(b)
+        assert torch.equal(want[f"{i}/rgb"], b["rgb"]) and torch.equal(want[f"{i}/depth"], b["depth"])
+        assert json.loads(str(want[f"{i}/im_infos"])) == b["im_infos"]
+        assert torch.equal(want[f"{i}/K"], b["cameras"].K)
         for k in ("gt_detections", "gt_data", "initial_data"):
-            if a[k] is None:
+            if bool(want[f"{i}/{k}/is_none"]):
                 assert b[k] is None
             else:
-                _same_collection(a[k], b[k])
-                assert a[k].poses.dtype == b[k].poses.dtype == torch.float32
+                a = helpers.StoredCollection(want, f"{i}/{k}")
+                _same_collection(a, b[k])
+                assert a.poses.dtype == b[k].poses.dtype == torch.float32
 
 
-@pytest.mark.reference
 @pytest.mark.parametrize("mode", ["gt", "external", "depth_refiner"])
-def test_runner_matches_the_reference_runner(ref_caller, mode, monkeypatch):
+def test_runner_matches_the_reference_runner(mode, monkeypatch):
     """Same frames, same stand-in estimator, the reference's PredictionRunner against ours: per-key predictions equal (but
     for our extra `time` column), same frame order, the first frame run twice (warm-up) by both."""
     obs = make_observations(5, with_init=(mode == "external"))
     cfg = InferenceConfig(**{**CFG.__dict__, **dict(coarse_estimation_type="external" if mode == "external" else "SO3_grid",
                                                     run_depth_refiner=(mode == "depth_refiner"))})
-    R = ref_caller
 
-    class RefDataset(R.scene_dataset.SceneDataset):
-        def __init__(self):
-            super().__init__(pd.DataFrame(dict(scene_id=[o.infos.scene_id for o in obs], view_id=[o.infos.view_id for o in obs])),
-                             load_depth=True)
+    def reference():
+        R = _ref_caller()
 
-        def _load_scene_observation(self, infos):
-            o = next(o for o in obs if (o.infos.scene_id, o.infos.view_id) == (infos.scene_id, infos.view_id))
-            return _to_reference_observation(R, o)
+        class RefDataset(R.scene_dataset.SceneDataset):
+            def __init__(self):
+                super().__init__(pd.DataFrame(dict(scene_id=[o.infos.scene_id for o in obs],
+                                                   view_id=[o.infos.view_id for o in obs])), load_depth=True)
 
-    # device moves of the reference (hard-coded .cuda()) -> identity on this CPU-only machine
-    monkeypatch.setattr(R.ns.tensor_collection.TensorCollection, "cuda", lambda self: self)
-    monkeypatch.setattr(R.ns.types.ObservationTensor, "cuda", lambda self, *a: self)
-    if mode == "external":
-        # the reference helper relies on groupby().apply() keeping the grouping columns (true for the pandas it pins, not for
-        # the one installed here, see tests/test_product_vs_reference.py): put them back after the reference's own call
-        U = sys.modules["megapose.inference.utils"]
-        original = U.add_instance_id
+            def _load_scene_observation(self, infos):
+                o = next(o for o in obs if (o.infos.scene_id, o.infos.view_id) == (infos.scene_id, infos.view_id))
+                return _to_reference_observation(R, o)
 
-        def add_instance_id(inputs):
-            before = inputs.infos[["batch_im_id", "label"]].copy()
-            out = original(inputs)
-            for c in before:
-                if c not in out.infos:
-                    out.infos[c] = before[c]
-            return out
+        # device moves of the reference (hard-coded .cuda()) -> identity on a CPU-only machine
+        monkeypatch.setattr(R.ns.tensor_collection.TensorCollection, "cuda", lambda self: self)
+        monkeypatch.setattr(R.ns.types.ObservationTensor, "cuda", lambda self, *a: self)
+        if mode == "external":
+            # the reference helper relies on groupby().apply() keeping the grouping columns (true for the pandas it pins,
+            # not for newer ones, see tests/test_product_vs_reference.py): put them back after the reference's own call
+            U = sys.modules["megapose.inference.utils"]
+            original = U.add_instance_id
 
-        monkeypatch.setattr(U, "add_instance_id", add_instance_id)
-    ref_cfg = R.ns.types.InferenceConfig(**cfg.__dict__)
-    ref_runner = R.prediction_runner.PredictionRunner(RefDataset(), ref_cfg, batch_size=1, n_workers=0)
-    est_a, est_b = StandInEstimator(), StandInEstimator()
-    want = ref_runner.get_predictions(est_a)
+            def add_instance_id(inputs):
+                before = inputs.infos[["batch_im_id", "label"]].copy()
+                out = original(inputs)
+                for c in before:
+                    if c not in out.infos:
+                        out.infos[c] = before[c]
+                return out
+
+            monkeypatch.setattr(U, "add_instance_id", add_instance_id)
+        ref_cfg = R.ns.types.InferenceConfig(**cfg.__dict__)
+        ref_runner = R.prediction_runner.PredictionRunner(RefDataset(), ref_cfg, batch_size=1, n_workers=0)
+        est_a = StandInEstimator()
+        preds = ref_runner.get_predictions(est_a)
+        out = dict(keys=helpers.json_array(sorted(preds)), calls=helpers.json_array(est_a.calls))
+        for k, v in preds.items():
+            out.update(helpers.collection_arrays(f"pred/{k}", v))
+        return out
+
+    stored = helpers.reference_outputs(f"prediction_runner_{mode}", reference)
+    est_b = StandInEstimator()
     runner = pr.PredictionRunner(pr.ListSceneDataset(obs, load_depth=True), cfg, device="cpu")
     got = runner.get_predictions(est_b)
-    assert est_a.calls == est_b.calls and len(est_b.calls) == len(obs) + 1
-    assert set(want) == set(got)
-    for k in want:
-        _same_collection(want[k], got[k])
+    assert json.loads(str(stored["calls"])) == json.loads(json.dumps(est_b.calls)) and len(est_b.calls) == len(obs) + 1
+    keys = json.loads(str(stored["keys"]))
+    assert set(keys) == set(got)
+    for k in keys:
+        _same_collection(helpers.StoredCollection(stored, f"pred/{k}"), got[k])
         assert "time" in got[k].infos
     assert [(t["scene_id"], t["view_id"]) for t in runner.frame_times] == \
         [(obs[i].infos.scene_id, obs[i].infos.view_id) for i in runner.sampler]
 
 
-@pytest.mark.reference
 def test_bop_csv_matches_the_toolkit_writer(tmp_path):
     """Byte-for-byte against the BOP toolkit's `inout.save_bop_results` as vendored by the reference."""
-    for name in ("imageio", "png"):
-        sys.modules.setdefault(name, types.ModuleType(name))
-    pkg = types.ModuleType("bop_toolkit_lib")
-    pkg.__path__ = []
-    pkg.misc = types.ModuleType("bop_toolkit_lib.misc")
-    sys.modules.setdefault("bop_toolkit_lib", pkg)
-    sys.modules.setdefault("bop_toolkit_lib.misc", pkg.misc)
-    spec = importlib.util.spec_from_file_location(
-        "bop_toolkit_lib_inout_ref", "/root/reference/deps/bop_toolkit_challenge/bop_toolkit_lib/inout.py")
-    inout = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(inout)
     preds = _predictions(7)
     rows = pr.predictions_to_bop(preds)
-    inout.save_bop_results(str(tmp_path / "ref.csv"), rows)
+
+    def reference():
+        from oracle import refload
+
+        for name in ("imageio", "png"):
+            sys.modules.setdefault(name, types.ModuleType(name))
+        pkg = types.ModuleType("bop_toolkit_lib")
+        pkg.__path__ = []
+        pkg.misc = types.ModuleType("bop_toolkit_lib.misc")
+        sys.modules.setdefault("bop_toolkit_lib", pkg)
+        sys.modules.setdefault("bop_toolkit_lib.misc", pkg.misc)
+        spec = importlib.util.spec_from_file_location(
+            "bop_toolkit_lib_inout_ref", refload.REF_ROOT.parents[1] / "deps/bop_toolkit_challenge/bop_toolkit_lib/inout.py")
+        inout = importlib.util.module_from_spec(spec)
+        spec.loader.exec_module(inout)
+        inout.save_bop_results(str(tmp_path / "ref.csv"), rows)
+        return dict(csv=np.frombuffer((tmp_path / "ref.csv").read_bytes(), dtype=np.uint8))
+
+    want = helpers.reference_outputs("bop_csv", reference)["csv"].numpy().tobytes()
     pr.save_bop_results(tmp_path / "mine.csv", rows)
-    assert (tmp_path / "ref.csv").read_bytes() == (tmp_path / "mine.csv").read_bytes()
+    assert want == (tmp_path / "mine.csv").read_bytes()
 
 
 # ------------------------------------------------------------------------------------------ no reference needed

@@ -23,7 +23,7 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--slots", default="2")
     ap.add_argument("--priority", default="0,1")
-    ap.add_argument("--conv-modes", default="60866571", help="comma-separated mpx_conv_set_mode values (set before building)")
+    ap.add_argument("--conv-modes", default="8", help="comma-separated mpx_conv_set_mode values (set before building)")
     ap.add_argument("--out", type=Path, default=Path("gpurun_out/frames_in_flight.json"))
     args = ap.parse_args()
     sc = scenes.bench_scene(1)

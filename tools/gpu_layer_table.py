@@ -1,12 +1,12 @@
-"""Per-layer table: every distinct convolution of the ResNet-34 coarse forward at batch 576, this library's tcgen05
-kernels next to stock torch / cuDNN on the same GPU (the "existing Blackwell kernel" bar of SURVEY 8d, VERDICT r1 item 2).
+"""Per-layer table: every distinct convolution of the ResNet-34 coarse forward at batch 576, this library's wgmma
+kernel next to stock torch / cuDNN on the same GPU (the vendor-library bar of SURVEY 8d).
 
     python tools/gpu_layer_table.py --out gpurun_out/layer_table.json [--batch 576] [--render-size 240x320]
 
 torch side: F.conv2d + folded-BN bias + (residual) + ReLU as separate ops is what eager PyTorch runs, but to give cuDNN
 its best case only the convolution itself is timed (bias / residual / ReLU / BN are free for it); the mpx side times the
 whole fused layer (conv + bias + residual + ReLU + 16-bit store).  CUDA events, L2 flushed by size (the activation
-tensors of every layer at batch 576 exceed the 126 MB L2 except in layer4).  Also prints the whole-network forward of
+tensors of every layer at batch 576 are as large as the 50 MB L2 or larger).  Also prints the whole-network forward of
 both sides (workloads/torch_resnet.py vs ResNet34Engine)."""
 import argparse
 import json

@@ -1,4 +1,4 @@
-"""The reference's network through stock PyTorch (cuDNN / cuBLAS) -- the "existing Blackwell kernel" bar of SURVEY 8(d).
+"""The reference's network through stock PyTorch (cuDNN / cuBLAS) -- the vendor-library bar of SURVEY 8(d).
 
 `TorchResNet34` is `resnet34(num_classes=512, n_input_channels=C)` + the single linear head
 (models/torchvision_resnet.py:181-316, models/pose_rigid.py:120-130, 314-334) as a plain nn.Module loaded from a
