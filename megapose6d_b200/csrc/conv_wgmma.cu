@@ -597,9 +597,10 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
   int block_n = block_n_override;
   if (block_n <= 0) {
     // wide tiles amortise the activation loads; with only a handful of output tiles (refiner: one sample) the
-    // conv is bound by the serial K loop of a single tile instead, so narrower tiles spread it over more SMs
+    // conv is bound by the serial K loop of a single tile instead, so narrower tiles spread it over more SMs.
+    // Start from the widest tile that divides C_out (C_out = 192, 320, 448: 64; 384: 128); halving keeps dividing it.
     const long long m_tiles_est = (M_total + kBlockM - 1) / kBlockM;
-    block_n = d.C_out >= 256 ? 256 : d.C_out;
+    block_n = d.C_out % 256 == 0 ? 256 : (d.C_out % 128 == 0 ? 128 : 64);
     while (block_n > 64 && m_tiles_est * (d.C_out / block_n) < 32) block_n /= 2;
   }
   MPX_REQUIRE((block_n == 64 || block_n == 128 || block_n == 256) && d.C_out % block_n == 0,

@@ -2,7 +2,9 @@
 
 The kernel-selection values of mpx_conv_set_mode that chose between kernel variants (window kernels, CTA pairs, staged
 epilogues) are accepted and have no effect in this build: one kernel serves every shape.  The tests that run a shape under
-several of those values keep checking that the result does not depend on them, and each result against fp32 torch.
+several of those values check each result against fp32 torch on Gaussian data and, on integer operands, bit for bit
+against the exact float64 convolution under every one of those values (test_gpu_conv_exact.py: how the operands are chosen,
+and the kernel's tile, pipeline, split-K and im2col edges).
 
 Tolerances (stated, floating point):
   * single conv vs fp32 torch conv on the same 16-bit-rounded operands: |err| <= ULP * max|ref| + ATOL, one rounding
@@ -22,6 +24,7 @@ from megapose6d_b200 import _abi
 from megapose6d_b200.backbone import ResNet34Engine
 from oracle import resnet_ref
 from tests import helpers
+from tests import test_gpu_conv_exact as conv_exact
 
 pytestmark = pytest.mark.gpu
 ACT = _abi.act_dtype() if torch.cuda.is_available() else torch.float16
@@ -29,6 +32,18 @@ ULP, ATOL = (2 ** -10, 2e-3) if ACT == torch.float16 else (2 ** -7, 1e-2)
 SINGLE_CTA_MODE = 11  # kernel-variant bits 0, 1 and split-K in the network (bit 3)
 DEFAULT_CONV_MODE = 8  # the library's default (include/mpx.h): split-K in the network for small batches
 RELOAD_MODE = DEFAULT_CONV_MODE | 32768  # a kernel-variant bit: no effect
+
+
+def _assert_bit_exact_under_modes(case, modes):
+    """`case` (a conv_exact.Conv) on integer operands: under every mode value the output equals the exact float64
+    convolution rounded to the 16-bit type."""
+    x, w, b, r, want = conv_exact._problem(case, conv_exact._gen(case.name))
+    try:
+        for mode in modes:
+            _abi.lib().mpx_conv_set_mode(mode)
+            assert torch.equal(conv_exact._launch(case, x, w, b, r), want), mode
+    finally:
+        _abi.lib().mpx_conv_set_mode(DEFAULT_CONV_MODE)
 
 
 def _conv_ref(x, w, bias, stride, pads, relu, residual):
@@ -224,6 +239,7 @@ def test_window_and_im2col_kernels_agree(case):
     tol = ULP * ref.abs().max().item() + ATOL
     assert (outs[0] - ref).abs().max() <= tol and (outs[1] - ref).abs().max() <= tol
     assert (outs[0] - outs[1]).abs().max() <= tol
+    _assert_bit_exact_under_modes(conv_exact.Conv(name, n, h, w, 64, 64, r, s, pads=pads, relu=relu, res=use_res), (1, 0))
 
 
 @pytest.mark.parametrize("cfg_name,n", [("refiner", 1), ("coarse", 2), ("refiner", 5)])
@@ -294,6 +310,8 @@ def test_layer2_window_kernel_agrees_with_im2col_and_torch(case):
     assert (outs[0] - ref).abs().max() <= tol and (outs[1] - ref).abs().max() <= tol
     # equal up to one 16-bit rounding
     assert (outs[0] - outs[1]).abs().max() <= ULP * ref.abs().max().item()
+    _assert_bit_exact_under_modes(conv_exact.Conv(name, n, h, w, 128, 128, 3, 3, pads=(1, 1, 1, 1), relu=relu, res=use_res,
+                                                  max_ctas=max_ctas), (SINGLE_CTA_MODE, SINGLE_CTA_MODE | 256))
 
 
 def test_graph_replay_equals_eager_launches():
@@ -354,6 +372,8 @@ def test_cta_pair_kernel_vs_torch_and_single_cta(case):
     assert (outs[0] - ref).abs().max() <= tol and (outs[1] - ref).abs().max() <= tol
     assert torch.equal(outs[0], outs[1])  # same products, same K order, fp32 accumulation
     assert torch.equal(outs[0], outs[2])  # staged epilogue (residual by TMA, bias from global memory): same arithmetic
+    _assert_bit_exact_under_modes(conv_exact.Conv(name, n, h, w, cin, cout, r, s, stride=stride, pads=pads, relu=relu,
+                                                  res=use_res), (7, 1, 7 | 33554432))
 
 
 PAIR_WINDOW_CASES = [
@@ -399,6 +419,9 @@ def test_layer2_pair_window_kernel(case):
         assert (o - ref).abs().max() <= tol
         assert (o - outs[-1]).abs().max() <= ULP * ref.abs().max().item()
     assert torch.equal(outs[0], outs[1])  # staged (TMA residual, coalesced stores) vs row-per-thread epilogue: same arithmetic
+    _assert_bit_exact_under_modes(conv_exact.Conv(name, n, h, w, cin, cout, 3, 3, pads=(1, 1, 1, 1), relu=relu, res=use_res,
+                                                  max_ctas=max_ctas),
+                                  (DEFAULT_CONV_MODE, DEFAULT_CONV_MODE ^ 16777216, SINGLE_CTA_MODE))
 
 
 PAIR_WINDOW64_CASES = [
@@ -444,6 +467,8 @@ def test_pair_window64_kernel(case):
         assert (o - ref).abs().max() <= tol
         assert (o - outs[-1]).abs().max() <= ULP * ref.abs().max().item()
     assert torch.equal(outs[0], outs[1])  # sliding window: the same MMAs in the same order per output row
+    _assert_bit_exact_under_modes(conv_exact.Conv(name, n, h, w, 64, 64, r, r, pads=pads, relu=relu, res=use_res,
+                                                  max_ctas=max_ctas), (DEFAULT_CONV_MODE, RELOAD_MODE, SINGLE_CTA_MODE))
 
 
 @pytest.mark.parametrize("mode", [DEFAULT_CONV_MODE, SINGLE_CTA_MODE], ids=["cta_pairs", "single_cta"])
