@@ -229,13 +229,18 @@ int mpx_conv2d_splitk(const void* d_x, int n, int h, int w, int c_in, const void
                            void* d_out, int block_n, int splits, void* stream);
 
 /* convolution options, default 8.  One kernel serves every shape (TMA im2col + wgmma, 128-row tiles, 64/128/256-wide
- * tiles chosen from the shape); the bits choose how the network drives it:
+ * tiles chosen from the shape), except that C_out = 64 with at least 2 * mpx_sm_count() 256-pixel tiles (automatic tile
+ * width, no K split, no pooled epilogue) runs on a pixel-major kernel: 256 pixels on the wgmma N dimension, two consumer
+ * warpgroups taking alternate tiles, the epilogue staged through shared memory and stored by TMA, and the structurally
+ * zero k16 steps of the space-to-depth stem (relu bit 1, c_pad 16 or 32) skipped.  The bits:
  *   8   mpx_net_forward splits the K loop of the convolutions after the stem over a thread-block cluster for batches <= 64
  *   512 launch without programmatic dependent launch
  *   262144 / 524288 cap the automatic small-batch K split (bit 3) at 2 / 1 CTAs per tile: less SM time per layer at a higher
  *       latency (set before graphs are captured; the trade for two frames in flight, frame_pipeline.py)
  *   2097152 mpx_net_forward lets the stem's epilogue max-pool (mpx_conv2d relu bit 2) instead of storing the stem output and
  *       running mpx_maxpool3x3s2 on it; the outputs are identical
+ *   4194304 (bit 22) never use the pixel-major C_out = 64 kernel (the 128-row kernel serves those convolutions)
+ *   67108864 (bit 26) use the pixel-major C_out = 64 kernel for every convolution it can serve, whatever its size
  * Other bits are accepted and have no effect. */
 int mpx_conv_set_mode(int mode);
 

@@ -514,6 +514,262 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 }
 
 // ---------------------------------------------------------------------------------------------
+// C_out = 64: pixel-major kernel with ping-pong consumers and a TMA epilogue
+// ---------------------------------------------------------------------------------------------
+// D^T[64 ch, 256 px] = W[64, K] * X[256 px, K]^T: the weights are the wgmma A operand (one 64 x 64 box per k-block), the
+// activations the B operand (two 128-pixel im2col boxes into consecutive halves of one 256-row, 128B-swizzled tile), so
+// each k16 step is one m64n256k16 -- 4 KB of operand reads per 262144 MACs instead of 4 KB per 65536 with 64-wide tiles.
+// Warpgroup 0 is the TMA producer; warpgroups 1 and 2 take alternate 256-pixel tiles of the CTA's persistent sequence, so
+// one runs its epilogue while the other issues MMAs.  The epilogue goes through a per-warpgroup staging tile: the residual
+// is TMA-loaded into it while the mainloop runs, the result is written over it in place and TMA-stored (rows >= M_total
+// are clipped by the tensor map).
+constexpr int kC64Pixels = 256;
+constexpr int kC64Stages = 4;
+constexpr int kC64ActBytes = kC64Pixels * kBlockK * 2;  // 32 KiB
+constexpr int kC64WBytes = 64 * kBlockK * 2;            // 8 KiB
+constexpr int kC64StageBytes = kC64ActBytes + kC64WBytes;
+constexpr int kC64StagingBytes = kC64Pixels * 64 * 2;   // 32 KiB per consumer warpgroup
+constexpr int kC64SmemBytes = kC64Stages * kC64StageBytes + 2 * kC64StagingBytes + 1024 /*align slack*/ +
+                              128 /*barriers*/ + 256 /*bias*/;
+static_assert(kC64SmemBytes <= 227 * 1024, "conv64: shared memory budget");
+
+struct Conv64Params {
+  int M_total, P, Q, S, stride, pad_h, pad_w, cblocks, num_k_blocks, m_tiles;
+  int relu;
+  int has_residual;
+  const float* bias;
+};
+
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map),
+               "r"(smem_u32(smem)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// the 128 threads of consumer warpgroup `cw` (named barriers 2 and 3)
+__device__ __forceinline__ void warpgroup_sync(int cw) { asm volatile("bar.sync %0, 128;" ::"r"(2 + cw) : "memory"); }
+// mainloop hand-off between the consumer warpgroups (named barriers 4 and 5: 128 arrive + 128 wait)
+__device__ __forceinline__ void mainloop_turn_wait(int cw) { asm volatile("bar.sync %0, 256;" ::"r"(4 + cw) : "memory"); }
+__device__ __forceinline__ void mainloop_turn_pass(int cw) { asm volatile("bar.arrive %0, 256;" ::"r"(5 - cw) : "memory"); }
+
+// Space-to-depth 7x7 stem (megapose6d_b200/backbone.py: _stem_s2d): weight column (r, s, (dy*2+dx)*c_pad + c) holds the 7x7
+// tap (2r+dy-1, 2s+dx-1), zero when that lies outside 0..6.  Bit k of the result: k16 step k of k-block kb multiplies a
+// slice that is not structurally zero.  c_pad = 16 * cblocks, so step k covers channels 16 (4 cb + k) .. + 15, all in slice
+// (4 cb + k) / cblocks.
+__host__ __device__ __forceinline__ uint32_t stem_live_steps(int kb, int cblocks, int S) {
+  const int tap = kb / cblocks, cb = kb - tap * cblocks;
+  const int r = tap / S, s = tap - r * S;
+  uint32_t live = 0;
+  for (int k = 0; k < 4; ++k) {
+    const int slice = (4 * cb + k) / cblocks;
+    const int ky = 2 * r + (slice >> 1) - 1, kx = 2 * s + (slice & 1) - 1;
+    if (ky >= 0 && ky <= 6 && kx >= 0 && kx <= 6) live |= 1u << k;
+  }
+  return live;
+}
+
+// One k-block's MMAs as one chain: the k16 steps whose bit is set in `live`, between a fence and a commit.  `live` must fold
+// to a constant at every call site: a wgmma behind a run-time branch makes ptxas end each branch with its own commit and
+// add a dummy group at the join, so the next wgmma_wait<1> drains the tensor pipe every k-block.
+__device__ __forceinline__ void wgmma_kblock(uint32_t live, float (&acc)[128], uint64_t da, uint64_t db) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < kBlockK / 16; ++k)  // 16 act16 = 32 B inside the swizzle atom: +2 per step in the (addr >> 4) field
+    if (live & (1u << k)) wgmma_m64n256k16(acc, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), 1u);
+  wgmma_commit();
+}
+
+// kStemCblocks = 0: every k16 step is issued.  1 or 2: the weights are the space-to-depth stem's (relu bit 1, 4x4 taps,
+// c_pad = 16 * kStemCblocks), its 16 * kStemCblocks k-blocks are unrolled so that stem_live_steps folds to a constant per
+// k-block, and the structurally zero k16 steps are not issued.
+template <int kStemCblocks>
+__global__ void __launch_bounds__(kThreads, 1)
+conv64_wgmma_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
+                    const __grid_constant__ CUtensorMap map_res, const __grid_constant__ CUtensorMap map_out,
+                    const Conv64Params p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_x = smem;
+  uint8_t* smem_w = smem + kC64Stages * kC64ActBytes;
+  uint8_t* staging = smem + kC64Stages * kC64StageBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + 2 * kC64StagingBytes);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + kC64Stages;
+  uint64_t* res_bar = bars + 2 * kC64Stages;  // [2], one per consumer warpgroup
+  float* bias_s = reinterpret_cast<float*>(bars + 16);
+
+  const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);
+  const int nk = p.num_k_blocks;
+  for (int i = threadIdx.x; i < 64; i += blockDim.x) bias_s[i] = p.bias[i];
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_out) : "memory");
+    if (p.has_residual) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_res) : "memory");
+    for (int i = 0; i < kC64Stages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 4);  // one arrive per warp of the consuming warpgroup
+    }
+    mbar_init(&res_bar[0], 1);
+    mbar_init(&res_bar[1], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  pdl_trigger();
+  __syncthreads();
+  pdl_wait();
+
+  if (wg == 0) {
+    // ===================== TMA producer =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      const int pq = p.P * p.Q;
+      for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x) {
+        int base_w[2], base_h[2], img[2];
+        const int m0 = tile * kC64Pixels;
+        const bool second = m0 + kBlockM < p.M_total;  // a half past the last pixel is not loaded: its columns are clipped
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int m = m0 + hh * kBlockM;
+          img[hh] = m / pq;
+          const int rem = m - img[hh] * pq;
+          const int p0 = rem / p.Q;
+          base_w[hh] = (rem - p0 * p.Q) * p.stride - p.pad_w;
+          base_h[hh] = p0 * p.stride - p.pad_h;
+        }
+        const uint32_t bytes = (second ? kC64ActBytes : kC64ActBytes / 2) + kC64WBytes;
+        int tap = 0, cb = 0;
+        for (int kb = 0; kb < nk; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          mbar_expect_tx(&full_bar[stage], bytes);
+          const int r = tap / p.S;
+          const int s = tap - r * p.S;
+          uint8_t* dst = smem_x + stage * kC64ActBytes;
+          tma_load_im2col_4d(dst, &map_x, &full_bar[stage], cb * kBlockK, base_w[0], base_h[0], img[0],
+                             static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+          if (second)
+            tma_load_im2col_4d(dst + kATileBytes, &map_x, &full_bar[stage], cb * kBlockK, base_w[1], base_h[1], img[1],
+                               static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+          tma_load_2d(smem_w + stage * kC64WBytes, &map_w, &full_bar[stage], kb * kBlockK, 0);
+          if (++cb == p.cblocks) {
+            cb = 0;
+            ++tap;
+          }
+          if (++stage == kC64Stages) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers: wgmma + staged epilogue =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = wg - 1;
+    const int t = threadIdx.x & 127;
+    const int lane = threadIdx.x & 31;
+    const int q = lane >> 2;
+    // after the lane ^ 4 exchange this thread holds channels (c, c + 1) + 8 h of pixel 8 j + px
+    const int c = 16 * (t >> 5) + (q & ~1);
+    const int px = 2 * (lane & 3) + (q & 1);
+    const bool odd = (q & 1) != 0;
+    uint8_t* stage_buf = staging + cw * kC64StagingBytes;
+    int local = 0;
+    for (int i = cw, tile = blockIdx.x + cw * gridDim.x; tile < p.m_tiles; i += 2, tile += 2 * gridDim.x, ++local) {
+      const int m0 = tile * kC64Pixels;
+      if (p.has_residual && t == 0) {
+        bulk_wait_read_all();  // the previous tile's store has read the staging tile
+        mbar_expect_tx(&res_bar[cw], kC64StagingBytes);
+        tma_load_2d(stage_buf, &map_res, &res_bar[cw], 0, m0);
+      }
+      // stage / phase from the CTA's k-block counter (both warpgroups' tiles, in tile order); unsigned, since only the
+      // counter modulo 2 * kC64Stages matters and that survives wrap-around at 2^32
+      const uint32_t g = static_cast<uint32_t>(i) * static_cast<uint32_t>(nk);
+      int stage = static_cast<int>(g % kC64Stages);
+      uint32_t phase = (g / kC64Stages) & 1u;
+      float acc[128];
+#pragma unroll
+      for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+      // The mainloops take turns: this one starts once the other warpgroup has waited on every full barrier of the
+      // previous tile, so no waiter is ever more than one phase behind a barrier (parity waits cannot tell phases 0 and 2
+      // apart).  One arrive per following tile, so no arrival is left pending at exit.
+      if (i > 0) mainloop_turn_wait(cw);
+      int prev_stage = -1;
+      auto kblock = [&](uint32_t live) {
+        mbar_wait(&full_bar[stage], phase);
+        wgmma_kblock(live, acc, make_sw128_desc(smem_u32(smem_w + stage * kC64WBytes)),
+                     make_sw128_desc(smem_u32(smem_x + stage * kC64ActBytes)));
+        wgmma_wait<1>();
+        if (prev_stage >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+        }
+        prev_stage = stage;
+        if (++stage == kC64Stages) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      };
+      if constexpr (kStemCblocks > 0) {
+#pragma unroll
+        for (int kb = 0; kb < 16 * kStemCblocks; ++kb) kblock(stem_live_steps(kb, kStemCblocks, 4));
+      } else {
+#pragma unroll 1
+        for (int kb = 0; kb < nk; ++kb) kblock(0xFu);
+      }
+      if (tile + static_cast<int>(gridDim.x) < p.m_tiles) mainloop_turn_pass(cw);
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+      if (t == 0) bulk_wait_read_all();
+      warpgroup_sync(cw);
+      if (p.has_residual) mbar_wait(&res_bar[cw], static_cast<uint32_t>(local) & 1u);
+      const uint32_t sbase = smem_u32(stage_buf);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float2 b = *reinterpret_cast<const float2*>(bias_s + c + 8 * h);
+        const int chunk = (c + 8 * h) >> 3;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          const float other = __shfl_xor_sync(0xffffffffu, odd ? v0 : v1, 4);
+          float f0 = (odd ? other : v0) + b.x;
+          float f1 = (odd ? v1 : other) + b.y;
+          const int row = 8 * j + px;  // row & 7 == px
+          const uint32_t addr =
+              sbase + static_cast<uint32_t>(row * 128 + ((chunk ^ px) << 4) + ((c & 7) << 1));
+          if (p.has_residual) {
+            uint32_t rr;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rr) : "r"(addr) : "memory");
+            const float2 r = unpack_act2(rr);
+            f0 += r.x;
+            f1 += r.y;
+          }
+          if (p.relu) {
+            f0 = fmaxf(f0, 0.f);
+            f1 = fmaxf(f1, 0.f);
+          }
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_act2(f0, f1)) : "memory");
+        }
+      }
+      fence_proxy_async_smem();
+      warpgroup_sync(cw);
+      if (t == 0) {
+        tma_store_2d(&map_out, stage_buf, 0, m0);
+        bulk_commit();
+      }
+    }
+    if (t == 0) bulk_wait_all();
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Host side: tensor maps + launch
 // ---------------------------------------------------------------------------------------------
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
@@ -574,6 +830,104 @@ int conv_out_dim(int in, int pad_lo, int pad_hi, int k, int stride) {
   return (in + pad_lo + pad_hi - k) / stride + 1;
 }
 
+// im2col map of the activations, 128-pixel boxes of 64 channels.  Dims are innermost-first: {C, W, H, N}.
+static int encode_im2col_map(CUtensorMap* map, const ConvDesc& d, const void* x) {
+  cuuint64_t dims[4] = {static_cast<cuuint64_t>(d.C_in), static_cast<cuuint64_t>(d.W),
+                        static_cast<cuuint64_t>(d.H), static_cast<cuuint64_t>(d.n_img)};
+  cuuint64_t strides[3] = {static_cast<cuuint64_t>(d.C_in) * 2,
+                           static_cast<cuuint64_t>(d.W) * d.C_in * 2,
+                           static_cast<cuuint64_t>(d.H) * d.W * d.C_in * 2};
+  // Bounding box of the filter's *base* pixel (CUTLASS: lower = -pad_lo,
+  // upper = pad_hi - (filter-1)*dilation; cutlass/conv/collective/detail.hpp).
+  int lower[2] = {-d.pad_lo_w, -d.pad_lo_h};
+  int upper[2] = {d.pad_hi_w - (d.S - 1), d.pad_hi_h - (d.R - 1)};
+  cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(d.stride), static_cast<cuuint32_t>(d.stride), 1};
+  CUresult r = g_encode_im2col(map, kTmaActType, 4, const_cast<void*>(x),
+                               dims, strides, lower, upper, /*channelsPerPixel=*/kBlockK,
+                               /*pixelsPerColumn=*/kBlockM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  MPX_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeIm2col failed (%d)", static_cast<int>(r));
+  // Driver quirk (<= 13.1) for im2col maps over tensors smaller than 128 KiB: same fix-up as
+  // cute/atom/copy_traits_sm90_im2col.hpp.
+  int drv = 0;
+  cudaDriverGetVersion(&drv);
+  const size_t bytes = static_cast<size_t>(d.n_img) * d.H * d.W * d.C_in * 2;
+  if (drv <= 13010 && bytes < 131072) {
+    reinterpret_cast<uint64_t*>(map)[1] &= ~(1ull << 21);
+  }
+  return MPX_OK;
+}
+
+// row-major [rows, cols] act16 matrix, (box_cols x box_rows) boxes, 128B swizzle
+static int encode_2d_map(CUtensorMap* map, const void* ptr, cuuint64_t cols, cuuint64_t rows, int box_cols, int box_rows,
+                         CUtensorMapL2promotion promo) {
+  cuuint64_t dims[2] = {cols, rows};
+  cuuint64_t strides[1] = {cols * 2};
+  cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = g_encode_tiled(map, kTmaActType, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  MPX_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
+  return MPX_OK;
+}
+
+static int conv64_forward(const ConvDesc& d, const CUtensorMap& map_x, const void* w, const float* bias,
+                          const void* residual, void* out, int M_total, int P, int Q, int cap, cudaStream_t stream) {
+  const int K_total = d.R * d.S * d.C_in;
+  CUtensorMap map_w, map_res, map_out;
+  int rc = encode_2d_map(&map_w, w, K_total, 64, kBlockK, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  if (rc != MPX_OK) return rc;
+  rc = encode_2d_map(&map_out, out, 64, M_total, 64, kC64Pixels, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+  if (rc != MPX_OK) return rc;
+  map_res = map_out;
+  if (residual != nullptr) {
+    rc = encode_2d_map(&map_res, residual, 64, M_total, 64, kC64Pixels, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+    if (rc != MPX_OK) return rc;
+  }
+  Conv64Params p{};
+  p.M_total = M_total;
+  p.P = P;
+  p.Q = Q;
+  p.S = d.S;
+  p.stride = d.stride;
+  p.pad_h = d.pad_lo_h;
+  p.pad_w = d.pad_lo_w;
+  p.cblocks = d.C_in / kBlockK;
+  p.num_k_blocks = d.R * d.S * p.cblocks;
+  p.m_tiles = (M_total + kC64Pixels - 1) / kC64Pixels;
+  p.relu = d.relu;
+  p.has_residual = residual != nullptr;
+  p.bias = bias;
+  // the coarse / scoring (c_pad 16) and refiner (c_pad 32) stems skip their zero slices; wider c_pad issues every step
+  const int stem_cblocks = (d.s2d_stem && d.R == 4 && d.S == 4 && p.cblocks <= 2) ? p.cblocks : 0;
+  long long live_steps = 0;  // k16 steps issued per tile
+  for (int kb = 0; kb < p.num_k_blocks; ++kb)
+    live_steps += __builtin_popcount(stem_cblocks ? stem_live_steps(kb, p.cblocks, p.S) : 0xFu);
+
+  static bool attr_set = false;
+  if (!attr_set) {
+    MPX_CHECK_CUDA(cudaFuncSetAttribute(conv64_wgmma_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        kC64SmemBytes));
+    MPX_CHECK_CUDA(cudaFuncSetAttribute(conv64_wgmma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        kC64SmemBytes));
+    MPX_CHECK_CUDA(cudaFuncSetAttribute(conv64_wgmma_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        kC64SmemBytes));
+    attr_set = true;
+  }
+  const int grid = p.m_tiles < cap ? p.m_tiles : cap;
+  ProfileSlot* slot = profile_begin(stream);
+  void (*kernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, Conv64Params) =
+      stem_cblocks == 1 ? conv64_wgmma_kernel<1> : (stem_cblocks == 2 ? conv64_wgmma_kernel<2> : conv64_wgmma_kernel<0>);
+  MPX_CHECK_CUDA(launch_pdl(kernel, dim3(grid), dim3(kThreads), kC64SmemBytes, stream, 1, map_x, map_w, map_res, map_out,
+                            p));
+  MPX_CHECK_CUDA(cudaGetLastError());
+  ++g_launches;
+  profile_end(slot, stream, 2.0 * M_total * 64 * live_steps * 16);
+  return MPX_OK;
+}
+
 // x: [n_img, H, W, C_in] act16; w: [C_out, R*S*C_in] act16 ((r,s,c) ordered); bias fp32 [C_out];
 // residual/out: [n_img, P, Q, C_out] act16.
 int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* bias,
@@ -606,46 +960,29 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
   MPX_REQUIRE((block_n == 64 || block_n == 128 || block_n == 256) && d.C_out % block_n == 0,
               "conv: BLOCK_N=%d invalid for C_out=%d", block_n, d.C_out);
 
-  // --- activation map (im2col). Dims are innermost-first: {C, W, H, N}.
+  // --- activation map (im2col): 128-pixel boxes of 64 channels
   CUtensorMap map_a, map_b;
-  {
-    cuuint64_t dims[4] = {static_cast<cuuint64_t>(d.C_in), static_cast<cuuint64_t>(d.W),
-                          static_cast<cuuint64_t>(d.H), static_cast<cuuint64_t>(d.n_img)};
-    cuuint64_t strides[3] = {static_cast<cuuint64_t>(d.C_in) * 2,
-                             static_cast<cuuint64_t>(d.W) * d.C_in * 2,
-                             static_cast<cuuint64_t>(d.H) * d.W * d.C_in * 2};
-    // Bounding box of the filter's *base* pixel (CUTLASS: lower = -pad_lo,
-    // upper = pad_hi - (filter-1)*dilation; cutlass/conv/collective/detail.hpp).
-    int lower[2] = {-d.pad_lo_w, -d.pad_lo_h};
-    int upper[2] = {d.pad_hi_w - (d.S - 1), d.pad_hi_h - (d.R - 1)};
-    cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(d.stride), static_cast<cuuint32_t>(d.stride), 1};
-    CUresult r = g_encode_im2col(&map_a, kTmaActType, 4, const_cast<void*>(x),
-                                 dims, strides, lower, upper, /*channelsPerPixel=*/kBlockK,
-                                 /*pixelsPerColumn=*/kBlockM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                                 CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    MPX_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeIm2col failed (%d)", static_cast<int>(r));
-    // Driver quirk (<= 13.1) for im2col maps over tensors smaller than 128 KiB: same fix-up as
-    // cute/atom/copy_traits_sm90_im2col.hpp.
-    int drv = 0;
-    cudaDriverGetVersion(&drv);
-    const size_t bytes = static_cast<size_t>(d.n_img) * d.H * d.W * d.C_in * 2;
-    if (drv <= 13010 && bytes < 131072) {
-      reinterpret_cast<uint64_t*>(&map_a)[1] &= ~(1ull << 21);
-    }
+  rc = encode_im2col_map(&map_a, d, x);
+  if (rc != MPX_OK) return rc;
+
+  // C_out = 64 with enough 256-pixel tiles to give every CTA at least two (one per consumer warpgroup): the pixel-major
+  // kernel.  Mode bit 22 never takes it, bit 26 takes it whatever the size.
+  const bool aligned = (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(residual) & 15) == 0;
+  const long long tiles256 = (M_total + kC64Pixels - 1) / kC64Pixels;
+  const int cap = max_ctas > 0 ? max_ctas : sm_count();
+  if (d.C_out == 64 && block_n_override == 0 && splitk <= 0 && !d.pool && aligned && (g_conv_mode & 4194304) == 0 &&
+      ((g_conv_mode & 67108864) != 0 || tiles256 >= 2LL * cap)) {
+    // a heuristic K split (splitk < 0) only applies below 2 * SMs / 4 128-row tiles, far under this kernel's threshold;
+    // with bit 26 a shape it would split stays on the 128-row kernel
+    const long long m_tiles128 = (M_total + kBlockM - 1) / kBlockM;
+    const int nkb = d.R * d.S * (d.C_in / kBlockK);
+    if (!(splitk < 0 && m_tiles128 * 2 <= cap && nkb >= 8))
+      return conv64_forward(d, map_a, w, bias, residual, out, static_cast<int>(M_total), P, Q, cap, stream);
   }
-  {
-    const cuuint64_t K_total = static_cast<cuuint64_t>(d.R) * d.S * d.C_in;
-    cuuint64_t dims[2] = {K_total, static_cast<cuuint64_t>(d.C_out)};
-    cuuint64_t strides[1] = {K_total * 2};
-    cuuint32_t box[2] = {kBlockK, static_cast<cuuint32_t>(block_n)};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode_tiled(&map_b, kTmaActType, 2, const_cast<void*>(w), dims,
-                                strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    MPX_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
-  }
+
+  rc = encode_2d_map(&map_b, w, static_cast<cuuint64_t>(d.R) * d.S * d.C_in, d.C_out, kBlockK, block_n,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  if (rc != MPX_OK) return rc;
 
   ConvParams p{};
   p.M_total = static_cast<int>(M_total);
