@@ -124,6 +124,25 @@ int mpx_raster_render_fused(const mpx_meshdb* db, const int32_t* d_label_idx, co
                             const float* d_depth_norm_z, void* d_workspace, size_t workspace_bytes,
                             void* stream);
 
+/* multi-object scenes: Panda3dSceneRenderer.render_scene (panda3d_renderer/panda3d_scene_renderer.py:139-358, outputs
+ * CameraRenderingData, panda3d_renderer/types.py:43-125).  View v draws instances d_inst_offsets[v] ..
+ * d_inst_offsets[v+1]-1 (d_inst_offsets [n_views+1]), instance i = mesh d_inst_label[i] at pose d_inst_TCO[i] [16] in that
+ * view's camera frame, under d_K[v] [9], with one shared depth test.  Triangle t of the view's k-th instance has scene
+ * index (face counts of instances 0..k-1) + t, and the nearest fragment wins with ties to the lower scene index -- to the
+ * lower instance, then the lower triangle: a one-instance scene renders exactly what mpx_raster_render renders.
+ * d_inst_color [n_inst,3] (may be NULL): when its first component is >= 0 the instance's albedo (vertex colours and
+ * texture) is replaced by that colour (Panda3dObjectData.color).  Outputs (any may be NULL): d_rgb, d_normals
+ * [n_views,3,h,w], d_depth [n_views,1,h,w] as mpx_raster_render, d_inst_id [n_views,h,w] int32 = the instance's index
+ * within its view, -1 for background.  A non-finite pose or an unknown label: that instance draws nothing; non-finite K
+ * or no instances: the view is black with d_inst_id -1.  Malformed device offsets are clamped to [0, n_inst]; a view that
+ * still holds more than 1024 instances draws nothing.  Refused before any launch: flags other than bits 0-1 (point lights
+ * are not defined for scenes), n_inst > 1024 * n_views, up to 2^31 scene triangles per view, a workspace smaller than
+ * mpx_raster_workspace_bytes(h, w).  Views run in chunks of 2 x mpx_sm_count() on `stream`. */
+int mpx_raster_render_scene(const mpx_meshdb* db, int n_views, int n_inst, const int32_t* d_inst_offsets,
+                            const int32_t* d_inst_label, const float* d_inst_TCO, const float* d_inst_color,
+                            const float* d_K, int h, int w, uint32_t flags, float* d_rgb, float* d_normals,
+                            float* d_depth, int32_t* d_inst_id, void* d_workspace, size_t workspace_bytes, void* stream);
+
 /* single-view samples (coarse / scoring model, models/pose_rigid.py:634-708): crop + render in one pass.
  * Sample i renders (d_label_idx[i], d_TCO[i], d_K[i] = its crop intrinsics) and crops the observation
  * d_img_nhwc4[d_im_idx[i]] with d_boxes_crop[i] (roi_align as in mpx_roi_align); each pixel's complete channel

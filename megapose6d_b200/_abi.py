@@ -38,6 +38,8 @@ def _declare(lib: ctypes.CDLL) -> None:
     lib.mpx_raster_render.argtypes = [vp, vp, vp, vp, c_int, c_int, c_int, c_uint32, vp, vp, vp, vp, c_size_t, vp]
     lib.mpx_raster_render_fused.argtypes = [vp, vp, vp, vp, c_int, c_int, c_int, c_int, c_uint32, vp, c_int,
                                             c_int, c_int, vp, vp, c_size_t, vp]
+    lib.mpx_raster_render_scene.argtypes = [vp, c_int, c_int, vp, vp, vp, vp, vp, c_int, c_int, c_uint32, vp, vp, vp,
+                                            vp, vp, c_size_t, vp]
     lib.mpx_render_crop_fused.argtypes = [vp, vp, vp, vp, c_int, c_int, c_int, c_uint32, vp, c_int, c_int, c_int, vp,
                                           vp, c_int, vp, c_int, c_int, vp, vp, c_size_t, vp]
     lib.mpx_pose_init_autodepth.argtypes = [vp, c_int, vp, vp, vp, vp, c_int, vp, vp]
@@ -83,7 +85,7 @@ def _declare(lib: ctypes.CDLL) -> None:
 EXPORTS = [
     "mpx_abi_version", "mpx_act_dtype", "mpx_last_error", "mpx_launch_count", "mpx_set_sm_limit", "mpx_sm_count", "mpx_profile_enable", "mpx_profile_summary",
     "mpx_meshdb_create", "mpx_meshdb_destroy", "mpx_meshdb_set_textures",
-    "mpx_raster_workspace_bytes", "mpx_raster_set_mode", "mpx_raster_render", "mpx_raster_render_fused", "mpx_render_crop_fused",
+    "mpx_raster_workspace_bytes", "mpx_raster_set_mode", "mpx_raster_render", "mpx_raster_render_fused", "mpx_raster_render_scene", "mpx_render_crop_fused",
     "mpx_pose_init_autodepth", "mpx_normalize_T", "mpx_crop_geometry", "mpx_multiview_cameras",
     "mpx_pose_update", "mpx_topk_per_group", "mpx_image_to_nhwc4", "mpx_roi_align", "mpx_roi_align_fused",
     "mpx_net_input_bytes", "mpx_conv2d", "mpx_conv2d_splitk", "mpx_conv_set_mode", "mpx_maxpool3x3s2", "mpx_avgpool_linear",

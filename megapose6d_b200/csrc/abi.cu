@@ -176,6 +176,26 @@ int mpx_render_crop_fused(const mpx_meshdb* db, const int32_t* d_label_idx, cons
                        static_cast<cudaStream_t>(stream));
 }
 
+int mpx_raster_render_scene(const mpx_meshdb* db, int n_views, int n_inst, const int32_t* d_inst_offsets,
+                            const int32_t* d_inst_label, const float* d_inst_TCO, const float* d_inst_color,
+                            const float* d_K, int h, int w, uint32_t flags, float* d_rgb, float* d_normals,
+                            float* d_depth, int32_t* d_inst_id, void* d_workspace, size_t workspace_bytes, void* stream) {
+  MPX_NOT_NULL(db);
+  MPX_REQUIRE(n_views >= 0 && n_inst >= 0, "mpx_raster_render_scene: n_views=%d n_inst=%d", n_views, n_inst);
+  if (n_views > 0) {
+    MPX_NOT_NULL(d_inst_offsets);
+    MPX_NOT_NULL(d_K);
+    MPX_NOT_NULL(d_workspace);
+  }
+  if (n_inst > 0) {
+    MPX_NOT_NULL(d_inst_label);
+    MPX_NOT_NULL(d_inst_TCO);
+  }
+  return raster_scene_launch(db->db, n_views, n_inst, d_inst_offsets, d_inst_label, d_inst_TCO, d_inst_color, d_K, h, w,
+                             flags, d_rgb, d_normals, d_depth, d_inst_id, d_workspace, workspace_bytes,
+                             static_cast<cudaStream_t>(stream));
+}
+
 // ---- geometry ----
 int mpx_pose_init_autodepth(const float* d_points, int n_pts, const int32_t* d_label_idx, const float* d_bboxes,
                             const float* d_K, const float* d_R, int n, float* d_TCO, void* stream) {

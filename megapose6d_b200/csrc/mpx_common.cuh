@@ -258,6 +258,10 @@ int raster_set_red_only(int on);
 int raster_launch(const MeshDb* db, const int32_t* label_idx, const float* TCO, const float* K, int n_views,
                   int h, int w, unsigned flags, const RasterOut& out, void* workspace, size_t workspace_bytes,
                   cudaStream_t stream);
+int raster_scene_launch(const MeshDb* db, int n_views, int n_inst, const int32_t* inst_offsets, const int32_t* inst_label,
+                        const float* inst_TCO, const float* inst_color, const float* K, int h, int w, unsigned flags,
+                        float* rgb, float* normals, float* depth, int32_t* inst_id, void* workspace,
+                        size_t workspace_bytes, cudaStream_t stream);
 
 // geom.cu
 int pose_init_autodepth(const float* points, int n_pts, const int* label_idx, const float* bboxes,

@@ -219,15 +219,16 @@ __device__ __forceinline__ void raster_bbox(const TriSetup& t, int h, int w, int
   i1 = min(h - 1, (maxy - kHalf) >> kSubBits);
 }
 
+// key_id: the low 32 bits of the visibility key -- the triangle index within its mesh, or its scene index (scene renderer)
 template <typename W>
-__device__ __forceinline__ void emit_fragment(const TriSetup& t, W w0, W w1, W w2, int tri,
+__device__ __forceinline__ void emit_fragment(const TriSetup& t, W w0, W w1, W w2, int key_id,
                                               unsigned long long* __restrict__ cell) {
   if ((w0 | w1 | w2) < 0) return;
   float l0, l1, l2;
   const float iz = sample_iz(t, w0, w1, w2, l0, l1, l2);
   if (!(iz >= kIzMin && iz <= kIzMax)) return;
   const unsigned long long key =
-      (static_cast<unsigned long long>(~__float_as_uint(iz)) << 32) | static_cast<unsigned>(tri);
+      (static_cast<unsigned long long>(~__float_as_uint(iz)) << 32) | static_cast<unsigned>(key_id);
   // default: fire-and-forget reduction -- no dependent L2 read in the coverage loop (13.25 -> 13.06 ms per step, raster
   // microbench 8.17 -> 7.42 ms); mpx_raster_set_mode without bit 1 (2) restores read-then-atomic
   if (c_red_only) {
@@ -237,11 +238,11 @@ __device__ __forceinline__ void emit_fragment(const TriSetup& t, W w0, W w1, W w
   }
 }
 
-// (C) coverage of one triangle restricted to rows [row_lo, row_hi]; bounding boxes above kBigArea pixels are queued
-// for the CTA-wide path
+// (C) coverage of triangle `tri` of `faces` restricted to rows [row_lo, row_hi], its keys carrying `key_id`; bounding
+// boxes above kBigArea pixels are queued (by key id) for the CTA-wide path
 template <bool CACHED>
-__device__ __forceinline__ void cover_triangle(const VtxSrc& src, const int4* __restrict__ faces, int tri, int row_lo,
-                                               int row_hi, int h, int w, unsigned long long* __restrict__ vis,
+__device__ __forceinline__ void cover_triangle(const VtxSrc& src, const int4* __restrict__ faces, int tri, int key_id,
+                                               int row_lo, int row_hi, int h, int w, unsigned long long* __restrict__ vis,
                                                int* s_big_count, int* s_big) {
   const TriSetup t = load_tri<CACHED>(src, faces, tri);
   if (!t.ok) return;
@@ -254,7 +255,7 @@ __device__ __forceinline__ void cover_triangle(const VtxSrc& src, const int4* __
   if (area > kBigArea) {
     const int slot = atomicAdd(s_big_count, 1);
     if (slot < kBigQueue) {
-      s_big[slot] = tri;
+      s_big[slot] = key_id;
       return;
     }
   }
@@ -279,7 +280,7 @@ __device__ __forceinline__ void cover_triangle(const VtxSrc& src, const int4* __
       int w0 = s0, w1 = s1, w2 = s2;
       unsigned long long* row = vis + i * w;
       for (int j = j0; j <= j1; ++j) {
-        emit_fragment<int>(t, w0, w1, w2, tri, row + j);
+        emit_fragment<int>(t, w0, w1, w2, key_id, row + j);
         w0 += ex0; w1 += ex1; w2 += ex2;
       }
       s0 += ey0; s1 += ey1; s2 += ey2;
@@ -289,21 +290,34 @@ __device__ __forceinline__ void cover_triangle(const VtxSrc& src, const int4* __
   for (int i = i0; i <= i1; ++i) {
     long long w0 = r0, w1 = r1, w2 = r2;
     for (int j = j0; j <= j1; ++j) {
-      emit_fragment<long long>(t, w0, w1, w2, tri, vis + i * w + j);
+      emit_fragment<long long>(t, w0, w1, w2, key_id, vis + i * w + j);
       w0 += dx0; w1 += dx1; w2 += dx2;
     }
     r0 += dy0; r1 += dy1; r2 += dy2;
   }
 }
 
-// queued large triangles: the whole CTA shares each bounding box
-template <bool CACHED>
-__device__ __forceinline__ void cover_big_triangles(const VtxSrc& src, const int4* __restrict__ faces, int nbig,
-                                                    const int* s_big, int row_lo, int row_hi, int h, int w,
-                                                    unsigned long long* __restrict__ vis) {
+// A triangle named by its key id: where its vertices come from, its mesh's faces and its index among them
+struct TriRef {
+  VtxSrc src;
+  const int4* faces;
+  int tri;
+};
+// key id = triangle index of one mesh (the single-object kernels)
+struct MeshTris {
+  const VtxSrc& src;
+  const int4* faces;
+  __device__ __forceinline__ TriRef operator()(int key_id) const { return TriRef{src, faces, key_id}; }
+};
+
+// queued large triangles: the whole CTA shares each bounding box; `tri_of` maps a queued key id to its triangle
+template <bool CACHED, typename TriOf>
+__device__ __forceinline__ void cover_big_triangles(const TriOf& tri_of, int nbig, const int* s_big, int row_lo,
+                                                    int row_hi, int h, int w, unsigned long long* __restrict__ vis) {
   for (int b = 0; b < nbig; ++b) {
-    const int tri = s_big[b];
-    const TriSetup t = load_tri<CACHED>(src, faces, tri);
+    const int key_id = s_big[b];
+    const TriRef r = tri_of(key_id);
+    const TriSetup t = load_tri<CACHED>(r.src, r.faces, r.tri);
     int j0, j1, i0, i1;
     raster_bbox(t, h, w, j0, j1, i0, i1);
     i0 = max(i0, row_lo);
@@ -317,7 +331,7 @@ __device__ __forceinline__ void cover_big_triangles(const VtxSrc& src, const int
       long long w1 = edge_fn(t.cx, t.cy, t.ax, t.ay, px, py);
       long long w2 = edge_fn(t.ax, t.ay, t.bx, t.by, px, py);
       if (t.flip) { w0 = -w0; w1 = -w1; w2 = -w2; }
-      emit_fragment<long long>(t, w0, w1, w2, tri, vis + i * w + j);
+      emit_fragment<long long>(t, w0, w1, w2, key_id, vis + i * w + j);
     }
   }
 }
@@ -390,11 +404,11 @@ __device__ __forceinline__ ResolveCtx make_resolve_ctx(const RasterOut& out, int
   return c;
 }
 
-template <bool CACHED, bool TEXTURED>
+template <bool CACHED, bool TEXTURED, bool COLOR_OVERRIDE = false>
 __device__ __forceinline__ void resolve_pixel(const ResolveCtx& ctx, const VtxSrc& src, const int4* __restrict__ faces,
                                               const float4* __restrict__ vattr, const TexRef& texref,
                                               unsigned long long key, int view, int i, int j, int h, int w, bool q8,
-                                              bool gl_axes, const RasterOut& out) {
+                                              bool gl_axes, const RasterOut& out, const float* color = nullptr) {
   const int npix = ctx.npix;
   const int pix = i * w + j;
   const float* sR = src.sR;
@@ -440,6 +454,10 @@ __device__ __forceinline__ void resolve_pixel(const ResolveCtx& ctx, const VtxSr
       texture_sample(texref, tu, tv, tc);
 #pragma unroll
       for (int k = 0; k < 3; ++k) col[k] = texref.modulate ? __fmul_rn(tc[k], col[k]) : tc[k];
+    }
+    if (COLOR_OVERRIDE && color[0] >= 0.f) {  // scene renderer: the albedo replaced by the instance's colour
+#pragma unroll
+      for (int k = 0; k < 3; ++k) col[k] = color[k];
     }
     if (ctx.verts != nullptr) {
       // render_normals=False models: ambient 0.1 + six white point lights of 0.4 on the object's axes at 10 bounding radii
@@ -629,9 +647,9 @@ raster_kernel(const MeshDb db, const int* __restrict__ label_idx, const float* _
 
     // (C) triangles
     for (int tri = threadIdx.x; tri < nf; tri += blockDim.x)
-      cover_triangle<true>(src, faces, tri, row_lo, row_hi, h, w, vis, &s_big_count, s_big);
+      cover_triangle<true>(src, faces, tri, tri, row_lo, row_hi, h, w, vis, &s_big_count, s_big);
     __syncthreads();
-    cover_big_triangles<true>(src, faces, min(s_big_count, kBigQueue), s_big, row_lo, row_hi, h, w, vis);
+    cover_big_triangles<true>(MeshTris{src, faces}, min(s_big_count, kBigQueue), s_big, row_lo, row_hi, h, w, vis);
     __syncthreads();
 
     resolve_rows<true, TEXTURED>(src, faces, db.vattr + 2 * v_off,
@@ -678,9 +696,9 @@ raster_cover_kernel(const MeshDb db, const int* __restrict__ label_idx, const fl
   src.sR = sR;
   src.fx = sK[0]; src.cx = sK[1]; src.fy = sK[2]; src.cy = sK[3];
   for (int tri = part * kCoverThreads + threadIdx.x; tri < nf; tri += parts * kCoverThreads)
-    cover_triangle<false>(src, faces, tri, 0, h - 1, h, w, vis, &s_big_count, s_big);
+    cover_triangle<false>(src, faces, tri, tri, 0, h - 1, h, w, vis, &s_big_count, s_big);
   __syncthreads();
-  cover_big_triangles<false>(src, faces, min(s_big_count, kBigQueue), s_big, 0, h - 1, h, w, vis);
+  cover_big_triangles<false>(MeshTris{src, faces}, min(s_big_count, kBigQueue), s_big, 0, h - 1, h, w, vis);
 }
 
 template <bool TEXTURED>
@@ -713,6 +731,222 @@ raster_resolve_kernel(const MeshDb db, const int* __restrict__ label_idx, const 
                                 vis_all + static_cast<size_t>(view) * h * w, view, row_lo, row_hi, h, w, (flags & 1u) != 0,
                                 (flags & 2u) != 0, out, s_axis, (flags & 4u) != 0 && valid ? db.verts + 3 * v_off : nullptr,
                                 valid ? db.radius[lab] : 0.f);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Scene renderer: several posed instances per view with one shared visibility buffer
+// (reference: panda3d_renderer/panda3d_scene_renderer.py:139-358 render_scene).  Modelled on the scatter path: a cover
+// kernel spreads the view's SCENE triangles over `parts` CTAs, a resolve kernel shades the pixels.  Triangle t of instance
+// k has scene index s = (face counts of the valid instances before k) + t, and the keys carry s: the largest 1/z wins,
+// ties go to the lower instance, then to the lower triangle.  A one-instance scene therefore holds exactly the keys, and
+// produces exactly the pixels, of mpx_raster_render.  Contract restated in tests/scene_ref.c.
+// ---------------------------------------------------------------------------------------------
+constexpr int kSceneMaxInst = 1024;
+
+struct SceneIn {
+  const int* inst_offsets;  // [n_views+1]
+  const int* inst_label;    // [n_inst]
+  const float* inst_TCO;    // [n_inst,16]
+  const float* inst_color;  // [n_inst,3] or nullptr
+  const float* K;           // [n_views,9]
+  int n_inst;
+};
+
+// Shared-memory image of one view's instances (dynamic shared memory, n_cap = max instances per view):
+//   R [n_cap,12] pose rows, pre [n_cap+1] exclusive prefix of the face counts, lab [n_cap] label (-1: contributes nothing),
+//   col [n_cap,3] colour override (resolve only; first component < 0: none)
+__host__ __device__ inline size_t scene_smem_bytes(int n_cap, bool colors) {
+  return sizeof(float) * 12 * n_cap + sizeof(int) * (2 * n_cap + 1) + (colors ? sizeof(float) * 3 * n_cap : 0);
+}
+
+// exclusive prefix sum of s[0..n) in place, s[n] = total; called by every thread, blockDim a multiple of 32
+__device__ __forceinline__ void block_exclusive_scan(int* s, int n, int* s_warp) {
+  const int per = (n + blockDim.x - 1) / blockDim.x;
+  const int lo = threadIdx.x * per, hi = min(n, lo + per);
+  int sum = 0;
+  for (int i = lo; i < hi; ++i) sum += s[i];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  int incl = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  if (lane == 31) s_warp[wid] = incl;
+  __syncthreads();
+  if (wid == 0) {
+    int x = lane < nw ? s_warp[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, x, o);
+      if (lane >= o) x += t;
+    }
+    if (lane < nw) s_warp[lane] = x;
+  }
+  __syncthreads();
+  int run = incl - sum + (wid > 0 ? s_warp[wid - 1] : 0);
+  for (int i = lo; i < hi; ++i) {
+    const int c = s[i];
+    s[i] = run;
+    run += c;
+  }
+  if (threadIdx.x == 0) s[n] = s_warp[nw - 1];
+  __syncthreads();
+}
+
+// Stage view `view`'s instances; every thread calls it.  Returns the instance count: 0 for a view with non-finite K,
+// no instances, or malformed offsets (clamped to [0, n_inst]; more than n_cap instances = malformed).
+__device__ int stage_scene_view(const MeshDb& db, const SceneIn& in, int view, int n_cap, float* s_R, int* s_pre,
+                                int* s_lab, float* s_col, float* sK, int* s_cnt, int* s_warp) {
+  __shared__ int s_lo;
+  if (threadIdx.x == 0) {
+    const int lo = min(max(in.inst_offsets[view], 0), in.n_inst);
+    const int hi = min(max(in.inst_offsets[view + 1], lo), in.n_inst);
+    const float* Kv = in.K + 9 * view;
+    bool ok = hi - lo <= n_cap;
+    for (int i = 0; i < 9; ++i) ok = ok && finite_f(Kv[i]);
+    s_lo = lo;
+    *s_cnt = ok ? hi - lo : 0;
+    sK[0] = Kv[0]; sK[1] = Kv[2]; sK[2] = Kv[4]; sK[3] = Kv[5];
+  }
+  __syncthreads();
+  const int cnt = *s_cnt, lo = s_lo;
+  for (int k = threadIdx.x; k < cnt; k += blockDim.x) {
+    const int inst = lo + k;
+    const float* T = in.inst_TCO + 16 * static_cast<size_t>(inst);
+    bool ok = true;
+    for (int i = 0; i < 16; ++i) ok = ok && finite_f(T[i]);
+    const int lab = in.inst_label[inst];
+    ok = ok && lab >= 0 && lab < db.n_meshes;
+    for (int i = 0; i < 12; ++i) s_R[12 * k + i] = T[i];
+    s_lab[k] = ok ? lab : -1;
+    s_pre[k] = ok ? static_cast<int>(db.face_offsets[lab + 1] - db.face_offsets[lab]) : 0;
+    if (s_col != nullptr) {
+      const float* c = in.inst_color;
+      const bool has = c != nullptr && c[3 * static_cast<size_t>(inst)] >= 0.f;
+      for (int i = 0; i < 3; ++i) s_col[3 * k + i] = has ? c[3 * static_cast<size_t>(inst) + i] : -1.f;
+    }
+  }
+  __syncthreads();
+  block_exclusive_scan(s_pre, cnt, s_warp);
+  return cnt;
+}
+
+// scene index -> instance and triangle (the instance by binary search over the prefix of the face counts)
+struct SceneTris {
+  const float* verts;
+  const long long* vert_offsets;
+  const int4* faces4;
+  const long long* face_offsets;
+  const float* s_R;
+  const int* s_pre;
+  const int* s_lab;
+  int cnt;
+  float fx, cx, fy, cy;
+  __device__ __forceinline__ int instance(int s) const {  // largest k with pre[k] <= s; pre[k] <= s < pre[k+1]
+    int lo = 0, hi = cnt - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (s_pre[mid] <= s) lo = mid;
+      else hi = mid - 1;
+    }
+    return lo;
+  }
+  __device__ __forceinline__ TriRef at(int k, int s) const {
+    const int lab = s_lab[k];
+    TriRef r;
+    r.src.cache = nullptr;
+    r.src.verts = verts + 3 * vert_offsets[lab];
+    r.src.sR = s_R + 12 * k;
+    r.src.fx = fx; r.src.cx = cx; r.src.fy = fy; r.src.cy = cy;
+    r.faces = faces4 + face_offsets[lab];
+    r.tri = s - s_pre[k];
+    return r;
+  }
+  __device__ __forceinline__ TriRef operator()(int s) const { return at(instance(s), s); }
+};
+
+__device__ __forceinline__ SceneTris make_scene_tris(const MeshDb& db, const float* s_R, const int* s_pre, const int* s_lab,
+                                                     int cnt, const float* sK) {
+  return SceneTris{db.verts, db.vert_offsets, db.faces4, db.face_offsets, s_R, s_pre, s_lab, cnt,
+                   sK[0], sK[1], sK[2], sK[3]};
+}
+
+// grid = views of the chunk x parts; view = view0 + blockIdx.x / parts, its buffer vis_all[blockIdx.x / parts]
+__global__ void __launch_bounds__(kCoverThreads)
+scene_cover_kernel(const MeshDb db, const SceneIn in, int view0, int h, int w, unsigned long long* __restrict__ vis_all,
+                   int parts, int n_cap) {
+  extern __shared__ __align__(16) unsigned char s_dyn[];
+  float* s_R = reinterpret_cast<float*>(s_dyn);
+  int* s_pre = reinterpret_cast<int*>(s_R + 12 * n_cap);
+  int* s_lab = s_pre + n_cap + 1;
+  __shared__ float sK[4];
+  __shared__ int s_cnt;
+  __shared__ int s_warp[32];
+  __shared__ int s_big_count;
+  __shared__ int s_big[kBigQueue];
+  const int lv = blockIdx.x / parts, part = blockIdx.x - lv * parts;
+  if (threadIdx.x == 0) s_big_count = 0;
+  const int cnt = stage_scene_view(db, in, view0 + lv, n_cap, s_R, s_pre, s_lab, nullptr, sK, &s_cnt, s_warp);
+  if (cnt == 0) return;  // block-uniform
+  const int total = s_pre[cnt];
+  unsigned long long* vis = vis_all + static_cast<size_t>(lv) * h * w;
+  const SceneTris tris = make_scene_tris(db, s_R, s_pre, s_lab, cnt, sK);
+  for (int s = part * kCoverThreads + threadIdx.x; s < total; s += parts * kCoverThreads) {
+    const TriRef r = tris(s);
+    cover_triangle<false>(r.src, r.faces, r.tri, s, 0, h - 1, h, w, vis, &s_big_count, s_big);
+  }
+  __syncthreads();
+  cover_big_triangles<false>(tris, min(s_big_count, kBigQueue), s_big, 0, h - 1, h, w, vis);
+}
+
+// grid = views of the chunk x row strips; `out` and inst_id point at the chunk's first view
+template <bool TEXTURED>
+__global__ void __launch_bounds__(kRasterThreads, 2)
+scene_resolve_kernel(const MeshDb db, const SceneIn in, int view0, int h, int w, unsigned flags, RasterOut out,
+                     int* __restrict__ inst_id, const unsigned long long* __restrict__ vis_all, int strips, int n_cap) {
+  extern __shared__ __align__(16) unsigned char s_dyn[];
+  float* s_R = reinterpret_cast<float*>(s_dyn);
+  int* s_pre = reinterpret_cast<int*>(s_R + 12 * n_cap);
+  int* s_lab = s_pre + n_cap + 1;
+  float* s_col = reinterpret_cast<float*>(s_lab + n_cap);
+  __shared__ float sK[4];
+  __shared__ int s_cnt;
+  __shared__ int s_warp[32];
+  const int lv = blockIdx.x / strips, strip = blockIdx.x - lv * strips;
+  const int rows_per_strip = (h + strips - 1) / strips;
+  const int row_lo = strip * rows_per_strip;
+  const int row_hi = min(h, row_lo + rows_per_strip) - 1;
+  const int cnt = stage_scene_view(db, in, view0 + lv, n_cap, s_R, s_pre, s_lab, s_col, sK, &s_cnt, s_warp);
+  const SceneTris tris = make_scene_tris(db, s_R, s_pre, s_lab, cnt, sK);
+  const bool q8 = (flags & 1u) != 0, gl_axes = (flags & 2u) != 0;
+  const ResolveCtx ctx = make_resolve_ctx(out, lv, h, w, nullptr);
+  const unsigned long long* vis = vis_all + static_cast<size_t>(lv) * h * w;
+  const int npix = h * w;
+  const TexRef no_tex{nullptr, nullptr, 0, 0, 0};
+  for (int pix = row_lo * w + threadIdx.x; pix < (row_hi + 1) * w; pix += blockDim.x) {
+    const int i = pix / w, j = pix - i * w;
+    const unsigned long long key = __ldcg(vis + pix);
+    int k = -1;
+    if (key == ~0ull) {  // background: no instance is looked up
+      VtxSrc none;
+      none.cache = nullptr; none.verts = nullptr; none.sR = s_R;
+      none.fx = none.cx = none.fy = none.cy = 0.f;
+      resolve_pixel<false, false>(ctx, none, db.faces4, db.vattr, no_tex, key, lv, i, j, h, w, q8, gl_axes, out);
+    } else {
+      const int s = static_cast<int>(key & 0xffffffffu);
+      k = tris.instance(s);
+      const TriRef r = tris.at(k, s);
+      const int lab = s_lab[k];
+      const long long v_off = db.vert_offsets[lab];
+      // the key the single-object renderer holds for this pixel: same 1/z bits, instance-local triangle index
+      const unsigned long long local = (key & 0xffffffff00000000ull) | static_cast<unsigned>(r.tri);
+      resolve_pixel<false, TEXTURED, true>(ctx, r.src, r.faces, db.vattr + 2 * v_off,
+                                           TEXTURED ? mesh_texture(db, lab, v_off, true) : no_tex, local, lv, i, j, h, w,
+                                           q8, gl_axes, out, s_col + 3 * k);
+    }
+    if (inst_id != nullptr) inst_id[static_cast<size_t>(lv) * npix + pix] = k;
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1240,6 +1474,63 @@ int raster_launch(const MeshDb* db, const int32_t* label_idx, const float* TCO, 
                                                               reinterpret_cast<unsigned long long*>(workspace), strips);
   MPX_CHECK_CUDA(cudaGetLastError());
   ++g_launches;
+  return MPX_OK;
+}
+
+int raster_scene_launch(const MeshDb* db, int n_views, int n_inst, const int32_t* inst_offsets, const int32_t* inst_label,
+                        const float* inst_TCO, const float* inst_color, const float* K, int h, int w, unsigned flags,
+                        float* rgb, float* normals, float* depth, int32_t* inst_id, void* workspace,
+                        size_t workspace_bytes, cudaStream_t stream) {
+  MPX_REQUIRE(db != nullptr, "raster_scene: null mesh database");
+  MPX_REQUIRE(n_views >= 0 && n_inst >= 0, "raster_scene: n_views=%d n_inst=%d", n_views, n_inst);
+  MPX_REQUIRE(h > 0 && w > 0 && h <= 4096 && w <= 4096, "raster_scene: resolution %dx%d unsupported", h, w);
+  MPX_REQUIRE((flags & 4u) == 0, "raster_scene: point lights are not implemented for scenes (only white ambient light)");
+  MPX_REQUIRE((flags & ~3u) == 0, "raster_scene: flags 0x%x: only bits 0 (quantise) and 1 (GL normals)", flags);
+  MPX_REQUIRE(static_cast<long long>(n_inst) <= static_cast<long long>(kSceneMaxInst) * n_views,
+              "raster_scene: %d instances for %d views (at most %d per view)", n_inst, n_views, kSceneMaxInst);
+  MPX_REQUIRE(workspace_bytes >= raster_workspace_bytes(h, w), "raster_scene: workspace too small");
+  if (n_views == 0) return MPX_OK;
+  const int n_cap = n_inst < 1 ? 1 : (n_inst < kSceneMaxInst ? n_inst : kSceneMaxInst);
+  MPX_REQUIRE(static_cast<long long>(n_cap) * db->nf_max < (1ll << 31),
+              "raster_scene: %d instances of up to %d triangles reach 2^31 scene triangles", n_cap, db->nf_max);
+  const size_t smem_cover = scene_smem_bytes(n_cap, false), smem_resolve = scene_smem_bytes(n_cap, true);
+  auto resolve = db->tex_info != nullptr ? scene_resolve_kernel<true> : scene_resolve_kernel<false>;
+  MPX_CHECK_CUDA(cudaFuncSetAttribute(scene_cover_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      static_cast<int>(smem_cover)));
+  MPX_CHECK_CUDA(cudaFuncSetAttribute(resolve, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      static_cast<int>(smem_resolve)));
+  SceneIn in{inst_offsets, inst_label, inst_TCO, inst_color, K, n_inst};
+  const size_t npix = static_cast<size_t>(h) * w;
+  const int chunk = 2 * sm_count();  // the visibility buffers of raster_workspace_bytes
+  // triangles per view if every instance had the largest mesh: about two per cover thread
+  const long long tris_per_view = static_cast<long long>((n_inst + n_views - 1) / n_views) * db->nf_max;
+  unsigned long long* vis = reinterpret_cast<unsigned long long*>(workspace);
+  for (int v0 = 0; v0 < n_views; v0 += chunk) {
+    const int nv = n_views - v0 < chunk ? n_views - v0 : chunk;
+    MPX_CHECK_CUDA(cudaMemsetAsync(vis, 0xFF, static_cast<size_t>(nv) * npix * sizeof(unsigned long long), stream));
+    long long parts = (tris_per_view + 2 * kCoverThreads - 1) / (2 * kCoverThreads);
+    const int max_parts = 8 * sm_count() / nv > 1 ? 8 * sm_count() / nv : 1;
+    if (parts > max_parts) parts = max_parts;
+    if (parts < 1) parts = 1;
+    scene_cover_kernel<<<nv * static_cast<int>(parts), kCoverThreads, smem_cover, stream>>>(*db, in, v0, h, w, vis,
+                                                                                           static_cast<int>(parts), n_cap);
+    MPX_CHECK_CUDA(cudaGetLastError());
+    int strips = 2 * sm_count() / nv;
+    if (strips < 1) strips = 1;
+    if (strips > h) strips = h;
+    const int rows = (h + strips - 1) / strips;
+    strips = (h + rows - 1) / rows;  // no empty strips
+    RasterOut out;
+    memset(&out, 0, sizeof(out));
+    out.rgb = rgb ? rgb + static_cast<size_t>(v0) * 3 * npix : nullptr;
+    out.normals = normals ? normals + static_cast<size_t>(v0) * 3 * npix : nullptr;
+    out.depth = depth ? depth + static_cast<size_t>(v0) * npix : nullptr;
+    resolve<<<nv * strips, kRasterThreads, smem_resolve, stream>>>(*db, in, v0, h, w, flags, out,
+                                                                  inst_id ? inst_id + static_cast<size_t>(v0) * npix : nullptr,
+                                                                  vis, strips, n_cap);
+    MPX_CHECK_CUDA(cudaGetLastError());
+    g_launches += 2;
+  }
   return MPX_OK;
 }
 

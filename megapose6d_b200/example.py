@@ -7,7 +7,11 @@ Directory layout (the reference's): `image_rgb.png` (+ `image_depth.png`, uint16
 translation]` per object (datasets/scene_dataset.py:67-120).  The JSON structures are restated here with numpy only (the
 reference wraps them in pinocchio `Transform`s).
 
-    python -m megapose6d_b200.example <example_dir> --model megapose-1.0-RGB-multi-hypothesis
+    python -m megapose6d_b200.example <example_dir> --model megapose-1.0-RGB-multi-hypothesis [--vis-outputs]
+
+`--vis-outputs` then renders every estimated pose into the image (one scene, run_inference_on_example.py:151-193) and
+writes visualizations/{mesh_overlay, contour_overlay, all_results}.png; `--vis-only` does only that, from an existing
+outputs/object_data.json.
 """
 from __future__ import annotations
 
@@ -221,14 +225,95 @@ def run_inference(example_dir: Path, model_name: str, models_root: Optional[Path
     return output
 
 
+def get_mask_from_rgb(img: np.ndarray) -> np.ndarray:
+    """visualization/utils.py:47-53: a pixel belongs to the rendering when any channel is > 0."""
+    return (np.asarray(img) > 0).any(axis=-1)
+
+
+def make_mesh_overlay(rgb_input: np.ndarray, rgb_rendered: np.ndarray) -> np.ndarray:
+    """BokehPlotter.plot_overlay (visualization/bokeh_plotter.py:106-130): the image lightened where nothing is rendered,
+    the rendering lightened where it is."""
+    assert rgb_input.dtype == np.uint8 and rgb_rendered.dtype == np.uint8
+    mask = get_mask_from_rgb(rgb_rendered)
+    overlay = np.zeros_like(rgb_input).astype(np.float32)
+    overlay[~mask] = rgb_input[~mask] * 0.6 + 255 * 0.4
+    overlay[mask] = rgb_rendered[mask] * 0.8 + 255 * 0.2
+    return overlay.astype(np.uint8)
+
+
+def _box3(mask: np.ndarray, op) -> np.ndarray:
+    """3x3 box max (op = np.logical_or) or min (np.logical_and) of a boolean image, edges replicated."""
+    p = np.pad(mask, 1, mode="edge")
+    h, w = mask.shape
+    out = p[1:h + 1, 1:w + 1].copy()
+    for di in range(3):
+        for dj in range(3):
+            out = op(out, p[di:di + h, dj:dj + w])
+    return out
+
+
+def make_contour_overlay(img: np.ndarray, render: np.ndarray, color: Tuple[int, int, int] = (0, 255, 0),
+                         dilate_iterations: int = 1) -> dict:
+    """The silhouette of the rendering drawn on the image (what visualization/utils.py:55-83 draws): the mask's boundary
+    pixels -- in the mask, with a 3x3 neighbour outside it -- dilated `dilate_iterations` times with a 3x3 box and
+    painted `color`.  The boundary is computed directly, not with an edge detector."""
+    mask = get_mask_from_rgb(render)
+    contour = mask & ~_box3(mask, np.logical_and)
+    for _ in range(dilate_iterations):
+        contour = _box3(contour, np.logical_or)
+    out = np.copy(img)
+    out[contour] = color
+    return dict(img=out, mask=mask, contour=contour)
+
+
+def render_object_data(example_dir: Path, object_datas: List[ObjectData], resolution: Tuple[int, int],
+                       K: np.ndarray) -> np.ndarray:
+    """All estimated poses in one scene seen by the image's camera (TWC = I), white ambient light: rgb (h, w, 3) uint8."""
+    from .renderer import Panda3dLightData
+    from .scene_renderer import Panda3dCameraData, Panda3dObjectData, Panda3dSceneRenderer
+
+    renderer = Panda3dSceneRenderer(make_object_dataset(example_dir))
+    camera = Panda3dCameraData(K=K, resolution=resolution, TWC=np.eye(4))
+    objects = [Panda3dObjectData(label=o.label, TWO=o.TWO) for o in object_datas]
+    lights = [Panda3dLightData(light_type="ambient", color=(1.0, 1.0, 1.0, 1.0))]
+    return renderer.render_scene(objects, [camera], lights, render_depth=False, render_binary_mask=False,
+                                 render_normals=False, copy_arrays=True)[0].rgb
+
+
+def make_output_visualization(example_dir: Path) -> Path:
+    """run_inference_on_example.py:151-193: visualizations/{mesh_overlay, contour_overlay, all_results}.png from
+    outputs/object_data.json."""
+    from PIL import Image
+
+    example_dir = Path(example_dir)
+    rgb, _, camera = load_observation(example_dir, load_depth=False)
+    object_datas = load_object_data(example_dir / "outputs" / "object_data.json")
+    rendered = render_object_data(example_dir, object_datas, camera.resolution, camera.K)
+    mesh_overlay = make_mesh_overlay(rgb, rendered)
+    contour_overlay = make_contour_overlay(rgb, rendered, color=(0, 255, 0), dilate_iterations=1)["img"]
+    vis_dir = example_dir / "visualizations"
+    vis_dir.mkdir(exist_ok=True)
+    Image.fromarray(mesh_overlay).save(vis_dir / "mesh_overlay.png")
+    Image.fromarray(contour_overlay).save(vis_dir / "contour_overlay.png")
+    Image.fromarray(np.concatenate([rgb, contour_overlay, mesh_overlay], axis=1)).save(vis_dir / "all_results.png")
+    return vis_dir
+
+
 def main(argv: Optional[List[str]] = None) -> None:
     parser = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     parser.add_argument("example_dir", type=Path)
     parser.add_argument("--model", type=str, default="megapose-1.0-RGB-multi-hypothesis", choices=sorted(NAMED_MODELS))
     parser.add_argument("--models-root", type=Path, default=None, help="directory holding <run_id>/{config.yaml,checkpoint.pth.tar}")
+    parser.add_argument("--vis-outputs", action="store_true",
+                        help="also render the estimated poses and write visualizations/*.png")
+    parser.add_argument("--vis-only", action="store_true",
+                        help="only visualise an existing outputs/object_data.json (no inference)")
     args = parser.parse_args(argv)
-    out = run_inference(args.example_dir, args.model, args.models_root)
-    print(f"wrote {len(out)} pose(s) to {args.example_dir / 'outputs' / 'object_data.json'}")
+    if not args.vis_only:
+        out = run_inference(args.example_dir, args.model, args.models_root)
+        print(f"wrote {len(out)} pose(s) to {args.example_dir / 'outputs' / 'object_data.json'}")
+    if args.vis_outputs or args.vis_only:
+        print(f"wrote visualizations to {make_output_visualization(args.example_dir)}")
 
 
 if __name__ == "__main__":

@@ -199,3 +199,7 @@ class BatchRenderer:
 
 # name used by the reference's callers
 Panda3dBatchRenderer = BatchRenderer
+
+# the multi-object scene renderer (Panda3dSceneRenderer.render_scene) and its types
+from .scene_renderer import (CameraRenderingData, Panda3dCameraData, Panda3dObjectData,  # noqa: E402,F401
+                             Panda3dSceneRenderer)
