@@ -294,6 +294,48 @@ size_t mpx_net_workspace_bytes(const mpx_net* net, int n, int h, int w);
 int mpx_net_forward(const mpx_net* net, const void* d_x, int n, int h, int w, float* d_out,
                     void* d_workspace, size_t workspace_bytes, void* stream);
 
+/* ---- BOP 2019 pose errors ------------------------------------------------------------------------
+ * The pose-error functions of the BOP toolkit (bop_toolkit_lib/pose_error.py: vsd, mssd, mspd, add, adi), vendored by the
+ * reference under deps/bop_toolkit_challenge; megapose6d_b200/bop_eval.py drives them.  Lengths are millimetres.
+ *
+ * mpx_bop_vsd: Visible Surface Discrepancy with the "step" cost and "bop19" visibility.  Pair p compares estimate render
+ * d_depth_est[d_est_idx[p]] with ground-truth render d_depth_gt[d_gt_idx[p]] ([n_est|n_gt, h, w] float32 METRES, 0 = no
+ * surface, as mpx_raster_render writes them) on test image i = d_img_idx[p]: d_depth_test [n_img, h, w] raw uint16,
+ * d_depth_scale [n_img] (test depth in mm = fp32(raw) * fp32(scale)), d_K [n_img, 9] float64.  Renders are shared by every
+ * pair that names them.  d_diameter [n_pairs] float64 mm; h_taus [n_taus] (1..MPX_BOP_MAX_TAUS) host float64 tolerances
+ * as fractions of the diameter; delta in mm.  Outputs: d_counts [n_pairs, 2 + n_taus] int64 = {union, intersection, pixels
+ * of the intersection with |dist_gt - dist_est| / diameter >= tau_k}, d_err [n_pairs, n_taus] float64 =
+ * (count_k + union - intersection) / union, 1.0 when the union is empty, NaN for a pair whose indices are out of range.
+ * The float64 arithmetic is the toolkit's, in its order, without contraction: the errors are bit-identical to it on the same
+ * depth images.  Refused before any launch: n_pairs < 0, empty images, h * w >= 2^31, n_taus out of range, a NULL
+ * required pointer. */
+#define MPX_BOP_MAX_TAUS 16
+int mpx_bop_vsd(int n_pairs, int h, int w, const uint16_t* d_depth_test, int n_img, const float* d_depth_scale,
+                const double* d_K, const float* d_depth_est, int n_est, const float* d_depth_gt, int n_gt,
+                const int32_t* d_est_idx, const int32_t* d_gt_idx, const int32_t* d_img_idx, const double* d_diameter,
+                const double* h_taus, int n_taus, float delta, int64_t* d_counts, double* d_err, void* stream);
+
+/* mpx_bop_point_errors: d_err [n_pairs] float64 of `kind` for pairs of poses of model d_model_idx[p]:
+ *   MPX_BOP_MSSD  min over the model's symmetries of the max point distance (mm)
+ *   MPX_BOP_MSPD  min over the symmetries of the max distance of the projections under d_K [n_pairs, 9] (px)
+ *   MPX_BOP_ADD   mean point distance (identity symmetry only)
+ *   MPX_BOP_ADI   mean distance from each point in the gt pose to the nearest point in the estimated pose
+ * d_pts [n_pts_total, 3] float64 model points (mm), model m = rows d_pt_offsets[m] .. d_pt_offsets[m+1]-1
+ * (d_pt_offsets [n_models+1] int64); d_syms [n_syms_total, 12] float64 symmetry transforms (R row-major, t), model m = rows
+ * d_sym_offsets[m] .. d_sym_offsets[m+1]-1 (needed by MSSD / MSPD, the identity included); d_pose_est / d_pose_gt
+ * [n_pairs, 12] float64 (R row-major, t in mm).  d_sym_argmin [n_pairs] int32 (may be NULL): index of the minimising
+ * symmetry within the model's set, the first one on ties (0 for ADD / ADI).  A pair with an unknown model, no points or
+ * no symmetries gets NaN and -1; offsets are clamped to the totals.  Refused before any launch: an unknown kind,
+ * n_pairs < 0, n_models < 1, a NULL required pointer. */
+#define MPX_BOP_MSSD 0
+#define MPX_BOP_MSPD 1
+#define MPX_BOP_ADD 2
+#define MPX_BOP_ADI 3
+int mpx_bop_point_errors(int kind, int n_pairs, int n_models, const double* d_pts, const int64_t* d_pt_offsets,
+                         long long n_pts_total, const double* d_syms, const int64_t* d_sym_offsets, long long n_syms_total,
+                         const int32_t* d_model_idx, const double* d_pose_est, const double* d_pose_gt, const double* d_K,
+                         double* d_err, int32_t* d_sym_argmin, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -68,6 +68,10 @@ def _declare(lib: ctypes.CDLL) -> None:
     lib.mpx_net_workspace_bytes.argtypes = [vp, c_int, c_int, c_int]
     lib.mpx_net_workspace_bytes.restype = c_size_t
     lib.mpx_net_forward.argtypes = [vp, vp, c_int, c_int, c_int, vp, vp, c_size_t, vp]
+    lib.mpx_bop_vsd.argtypes = [c_int, c_int, c_int, vp, c_int, vp, vp, vp, c_int, vp, c_int, vp, vp, vp, vp, vp, c_int,
+                                c_float, vp, vp, vp]
+    lib.mpx_bop_point_errors.argtypes = [c_int, c_int, c_int, vp, vp, ctypes.c_longlong, vp, vp, ctypes.c_longlong, vp, vp,
+                                         vp, vp, vp, vp, vp]
     lib.mpx_launch_count.restype = ctypes.c_longlong
     lib.mpx_profile_enable.argtypes = [c_int]
     lib.mpx_set_sm_limit.argtypes = [c_int]
@@ -90,6 +94,7 @@ EXPORTS = [
     "mpx_pose_update", "mpx_topk_per_group", "mpx_image_to_nhwc4", "mpx_roi_align", "mpx_roi_align_fused",
     "mpx_net_input_bytes", "mpx_conv2d", "mpx_conv2d_splitk", "mpx_conv_set_mode", "mpx_maxpool3x3s2", "mpx_avgpool_linear",
     "mpx_net_create", "mpx_net_create_preact", "mpx_net_destroy", "mpx_net_set_graphs", "mpx_net_workspace_bytes", "mpx_net_forward",
+    "mpx_bop_vsd", "mpx_bop_point_errors",
 ]
 
 

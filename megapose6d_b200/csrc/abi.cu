@@ -454,4 +454,54 @@ int mpx_net_forward(const mpx_net* net, const void* d_x, int n, int h, int w, fl
                      static_cast<cudaStream_t>(stream));
 }
 
+// ---- BOP pose errors ----
+int mpx_bop_vsd(int n_pairs, int h, int w, const uint16_t* d_depth_test, int n_img, const float* d_depth_scale,
+                const double* d_K, const float* d_depth_est, int n_est, const float* d_depth_gt, int n_gt,
+                const int32_t* d_est_idx, const int32_t* d_gt_idx, const int32_t* d_img_idx, const double* d_diameter,
+                const double* h_taus, int n_taus, float delta, int64_t* d_counts, double* d_err, void* stream) {
+  MPX_REQUIRE(n_pairs >= 0, "mpx_bop_vsd: n_pairs=%d < 0", n_pairs);
+  MPX_REQUIRE(n_taus >= 1 && n_taus <= MPX_BOP_MAX_TAUS, "mpx_bop_vsd: n_taus=%d not in 1..%d", n_taus, MPX_BOP_MAX_TAUS);
+  MPX_NOT_NULL(h_taus);
+  if (n_pairs == 0) return MPX_OK;
+  MPX_REQUIRE(h > 0 && w > 0 && static_cast<long long>(h) * w < (1ll << 31), "mpx_bop_vsd: bad image size %dx%d", h, w);
+  MPX_REQUIRE(n_img > 0 && n_est > 0 && n_gt > 0, "mpx_bop_vsd: n_img=%d n_est=%d n_gt=%d", n_img, n_est, n_gt);
+  MPX_NOT_NULL(d_depth_test);
+  MPX_NOT_NULL(d_depth_scale);
+  MPX_NOT_NULL(d_K);
+  MPX_NOT_NULL(d_depth_est);
+  MPX_NOT_NULL(d_depth_gt);
+  MPX_NOT_NULL(d_est_idx);
+  MPX_NOT_NULL(d_gt_idx);
+  MPX_NOT_NULL(d_img_idx);
+  MPX_NOT_NULL(d_diameter);
+  MPX_NOT_NULL(d_counts);
+  MPX_NOT_NULL(d_err);
+  return bop_vsd(n_pairs, h, w, d_depth_test, n_img, d_depth_scale, d_K, d_depth_est, n_est, d_depth_gt, n_gt, d_est_idx,
+                 d_gt_idx, d_img_idx, d_diameter, h_taus, n_taus, delta, d_counts, d_err, static_cast<cudaStream_t>(stream));
+}
+
+int mpx_bop_point_errors(int kind, int n_pairs, int n_models, const double* d_pts, const int64_t* d_pt_offsets,
+                         long long n_pts_total, const double* d_syms, const int64_t* d_sym_offsets, long long n_syms_total,
+                         const int32_t* d_model_idx, const double* d_pose_est, const double* d_pose_gt, const double* d_K,
+                         double* d_err, int32_t* d_sym_argmin, void* stream) {
+  MPX_REQUIRE(kind >= MPX_BOP_MSSD && kind <= MPX_BOP_ADI, "mpx_bop_point_errors: unknown error kind %d", kind);
+  MPX_REQUIRE(n_pairs >= 0, "mpx_bop_point_errors: n_pairs=%d < 0", n_pairs);
+  if (n_pairs == 0) return MPX_OK;
+  MPX_REQUIRE(n_models >= 1 && n_pts_total >= 0 && n_syms_total >= 0, "mpx_bop_point_errors: n_models=%d", n_models);
+  MPX_NOT_NULL(d_pts);
+  MPX_NOT_NULL(d_pt_offsets);
+  MPX_NOT_NULL(d_model_idx);
+  MPX_NOT_NULL(d_pose_est);
+  MPX_NOT_NULL(d_pose_gt);
+  MPX_NOT_NULL(d_err);
+  if (kind == MPX_BOP_MSSD || kind == MPX_BOP_MSPD) {
+    MPX_NOT_NULL(d_syms);
+    MPX_NOT_NULL(d_sym_offsets);
+  }
+  if (kind == MPX_BOP_MSPD) MPX_NOT_NULL(d_K);
+  return bop_point_errors(kind, n_pairs, n_models, d_pts, d_pt_offsets, n_pts_total,
+                          (kind == MPX_BOP_MSSD || kind == MPX_BOP_MSPD) ? d_syms : nullptr, d_sym_offsets, n_syms_total,
+                          d_model_idx, d_pose_est, d_pose_gt, d_K, d_err, d_sym_argmin, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

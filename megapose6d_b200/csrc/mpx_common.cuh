@@ -288,4 +288,14 @@ int image_to_nhwc4(const float* in, int b, int c, int h, int w, float* out, cuda
 int roi_align_launch(const float* images, int b, int h, int w, const int* im_idx, const float* boxes, int n,
                      int c, int oh, int ow, const CropOut& out, cudaStream_t stream);
 
+// bop_eval.cu
+int bop_vsd(int n_pairs, int h, int w, const uint16_t* test, int n_img, const float* depth_scale, const double* K,
+            const float* dest, int n_est, const float* dgt, int n_gt, const int* est_idx, const int* gt_idx,
+            const int* img_idx, const double* diameter, const double* h_taus, int n_taus, float delta,
+            int64_t* counts, double* err, cudaStream_t stream);
+int bop_point_errors(int kind, int n_pairs, int n_models, const double* pts, const int64_t* pt_off, long long n_pts_total,
+                     const double* syms, const int64_t* sym_off, long long n_syms_total, const int* model_idx,
+                     const double* pose_est, const double* pose_gt, const double* K, double* err, int* sym_argmin,
+                     cudaStream_t stream);
+
 }  // namespace mpx
