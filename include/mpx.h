@@ -259,6 +259,10 @@ int mpx_conv2d_splitk(const void* d_x, int n, int h, int w, int c_in, const void
  *   2097152 mpx_net_forward lets the stem's epilogue max-pool (mpx_conv2d relu bit 2) instead of storing the stem output and
  *       running mpx_maxpool3x3s2 on it; the outputs are identical
  *   4194304 (bit 22) never use the pixel-major C_out = 64 kernel (the 128-row kernel serves those convolutions)
+ *   8388608 (bit 23) the pixel-major kernel loads its activations by im2col (every input pixel once per filter tap) for
+ *       every shape; by default a stride-1 convolution whose padded input row (W + both pads) is at most 256 pixels and
+ *       whose C_in is at most 128 loads one band of whole input rows per (filter row, 64 channels) instead and reuses
+ *       it over the filter's columns; the outputs are identical
  *   67108864 (bit 26) use the pixel-major C_out = 64 kernel for every convolution it can serve, whatever its size
  * Other bits are accepted and have no effect. */
 int mpx_conv_set_mode(int mode);

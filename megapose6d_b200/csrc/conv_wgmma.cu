@@ -115,16 +115,29 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_
       : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
 }
+__device__ __forceinline__ void wgmma_m64n160k16(float (&d)[80], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %82, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n160k16.f32." MPX_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, %80, %81, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
+      : "memory");
+}
 template <int BLOCK_N>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BLOCK_N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
   if constexpr (BLOCK_N == 64) wgmma_m64n64k16(d, da, db, accumulate);
   else if constexpr (BLOCK_N == 128) wgmma_m64n128k16(d, da, db, accumulate);
+  else if constexpr (BLOCK_N == 160) wgmma_m64n160k16(d, da, db, accumulate);
   else wgmma_m64n256k16(d, da, db, accumulate);
 }
 
 // K-major, 128-byte-swizzled operand tile (rows of 64 act16 = 128 B, 8-row groups 1024 B apart), as TMA writes it with
 // CU_TENSOR_MAP_SWIZZLE_128B.  wgmma descriptor: start>>4 [0,14), LBO>>4 [16,30) (unused for swizzled K-major),
-// SBO>>4 [32,46) = 1024 B, layout type [62,64) = 1 (128-byte swizzle).
+// SBO>>4 [32,46) = 1024 B, layout type [62,64) = 1 (128-byte swizzle).  The swizzle is applied to the absolute shared
+// address on sm_90a, so a tile may also start a whole number of 128-byte rows past a 1024-byte boundary (the band B
+// operand of conv64_wgmma_kernel) with the base-offset field [49,52) left at 0: measured on an H100, where setting that
+// field to (start >> 7) & 7 misreads every odd row shift.
 __device__ __forceinline__ uint64_t make_sw128_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
@@ -516,25 +529,45 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 // ---------------------------------------------------------------------------------------------
 // C_out = 64: pixel-major kernel with ping-pong consumers and a TMA epilogue
 // ---------------------------------------------------------------------------------------------
-// D^T[64 ch, 256 px] = W[64, K] * X[256 px, K]^T: the weights are the wgmma A operand (one 64 x 64 box per k-block), the
-// activations the B operand (two 128-pixel im2col boxes into consecutive halves of one 256-row, 128B-swizzled tile), so
-// each k16 step is one m64n256k16 -- 4 KB of operand reads per 262144 MACs instead of 4 KB per 65536 with 64-wide tiles.
-// Warpgroup 0 is the TMA producer; warpgroups 1 and 2 take alternate 256-pixel tiles of the CTA's persistent sequence, so
-// one runs its epilogue while the other issues MMAs.  The epilogue goes through a per-warpgroup staging tile: the residual
-// is TMA-loaded into it while the mainloop runs, the result is written over it in place and TMA-stored (rows >= M_total
-// are clipped by the tensor map).
+// D^T[64 ch, N px] = W[64, K] * X[N px, K]^T: the weights are the wgmma A operand (one 64 x 64 box per k-block), the
+// activations the B operand, so each k16 step is one m64nNk16 -- 4 KB of operand reads per 262144 MACs at N = 256
+// instead of 4 KB per 65536 with 64-wide tiles.  Two producers fill the B operand:
+//   im2col (kBandN = 0): a tile is 256 consecutive output pixels of the flattened NHW space; per k-block two 128-pixel
+//     im2col boxes fill one 256-row tile, so every input pixel is loaded once per filter tap.
+//   band (kBandN = 160 or 256, stride 1): a tile is `band_rows` whole output rows of one image.  Output pixel (j, q) of
+//     the tile is column j * Wp + q of a padded-width pixel space, Wp = Q + S - 1 = the padded input width, so tap (r, s)
+//     reads band pixel column + s of filter row r's band: the input rows p0 + r - pad_h .. + band_rows - 1, every padded
+//     column, loaded by one tiled TMA box per (filter row, cblock) with the padding zero-filled by the tensor map.  Tap s
+//     takes its B operand s rows (s * 128 B) into the band; columns q >= Q and rows past the tile are computed and dropped.
+//     The bands have a ring of their own (a tile holds `cblocks` of them at once: the (r, s, cblock, k) sum order of
+//     every output stays that of the im2col producer); the weights keep the per-k-block ring.
+// Warpgroup 0 is the TMA producer; warpgroups 1 and 2 take alternate tiles of the CTA's persistent sequence, so one runs
+// its epilogue while the other issues MMAs.  The epilogue goes through a per-warpgroup staging tile: the residual is
+// TMA-loaded into it while the mainloop runs, the result is written over it in place and TMA-stored (rows >= M_total, or
+// for band tiles rows >= P, are clipped by the tensor map).
 constexpr int kC64Pixels = 256;
 constexpr int kC64Stages = 4;
 constexpr int kC64ActBytes = kC64Pixels * kBlockK * 2;  // 32 KiB
 constexpr int kC64WBytes = 64 * kBlockK * 2;            // 8 KiB
 constexpr int kC64StageBytes = kC64ActBytes + kC64WBytes;
 constexpr int kC64StagingBytes = kC64Pixels * 64 * 2;   // 32 KiB per consumer warpgroup
-constexpr int kC64SmemBytes = kC64Stages * kC64StageBytes + 2 * kC64StagingBytes + 1024 /*align slack*/ +
-                              128 /*barriers*/ + 256 /*bias*/;
-static_assert(kC64SmemBytes <= 227 * 1024, "conv64: shared memory budget");
+// band producer: up to 3 band slots, then the weights (all k-blocks resident, or a ring of 8 stages), then the two
+// staging tiles; with the ring, the same 224 KiB as the im2col producer's stages and staging tiles
+constexpr int kC64BandSlots = 3;
+constexpr int kC64BandWStages = 8;
+static_assert(kC64BandSlots * kC64ActBytes + kC64BandWStages * kC64WBytes == kC64Stages * kC64StageBytes,
+              "conv64: the band producer's ring layout is the im2col producer's");
+constexpr int kC64SmemBytes = 227 * 1024;
+// stages / bands / weights / staging tiles in the first kC64BufferBytes, then 256 B of barriers and 256 B of bias
+constexpr int kC64BufferBytes = kC64SmemBytes - 1024 /*align slack*/ - 256 /*barriers*/ - 256 /*bias*/;
+static_assert(kC64Stages * kC64StageBytes + 2 * kC64StagingBytes <= kC64BufferBytes, "conv64: shared memory budget");
 
 struct Conv64Params {
   int M_total, P, Q, S, stride, pad_h, pad_w, cblocks, num_k_blocks, m_tiles;
+  int band_w, band_rows, tiles_per_img;  // band producer: Wp, output rows per tile, tiles per image
+  // band producer layout (bytes, multiples of 1024): band_slots slots of slot_bytes at 0, the weights at w_off (every
+  // k-block when w_resident, else a ring of kC64BandWStages), the two staging tiles of staging_bytes at staging_off
+  int band_slots, slot_bytes, w_resident, w_off, staging_off, staging_bytes;
   int relu;
   int has_residual;
   const float* bias;
@@ -543,6 +576,19 @@ struct Conv64Params {
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map),
                "r"(smem_u32(smem)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2,
+                                            int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(smem)),
+      "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, const void* smem, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(map),
+               "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
@@ -574,33 +620,44 @@ __host__ __device__ __forceinline__ uint32_t stem_live_steps(int kb, int cblocks
 // One k-block's MMAs as one chain: the k16 steps whose bit is set in `live`, between a fence and a commit.  `live` must fold
 // to a constant at every call site: a wgmma behind a run-time branch makes ptxas end each branch with its own commit and
 // add a dummy group at the join, so the next wgmma_wait<1> drains the tensor pipe every k-block.
-__device__ __forceinline__ void wgmma_kblock(uint32_t live, float (&acc)[128], uint64_t da, uint64_t db) {
+template <int N>
+__device__ __forceinline__ void wgmma_kblock(uint32_t live, float (&acc)[N / 2], uint64_t da, uint64_t db) {
   wgmma_fence();
 #pragma unroll
   for (int k = 0; k < kBlockK / 16; ++k)  // 16 act16 = 32 B inside the swizzle atom: +2 per step in the (addr >> 4) field
-    if (live & (1u << k)) wgmma_m64n256k16(acc, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), 1u);
+    if (live & (1u << k)) wgmma_tile<N>(acc, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), 1u);
   wgmma_commit();
 }
 
 // kStemCblocks = 0: every k16 step is issued.  1 or 2: the weights are the space-to-depth stem's (relu bit 1, 4x4 taps,
 // c_pad = 16 * kStemCblocks), its 16 * kStemCblocks k-blocks are unrolled so that stem_live_steps folds to a constant per
 // k-block, and the structurally zero k16 steps are not issued.
-template <int kStemCblocks>
+// kBandN = 0: the im2col producer; 160 or 256: the band producer with an m64n{kBandN}k16 chain per k16 step.
+template <int kStemCblocks, int kBandN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv64_wgmma_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w,
                     const __grid_constant__ CUtensorMap map_res, const __grid_constant__ CUtensorMap map_out,
                     const Conv64Params p) {
+  constexpr bool kBand = kBandN > 0;
+  constexpr int kN = kBand ? kBandN : kC64Pixels;            // wgmma N = accumulator columns per tile
+  constexpr int kStages = kBand ? kC64BandWStages : kC64Stages;  // ring of k-blocks (im2col: activations + weights)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_x = smem;
-  uint8_t* smem_w = smem + kC64Stages * kC64ActBytes;
-  uint8_t* staging = smem + kC64Stages * kC64StageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + 2 * kC64StagingBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + kC64Stages;
-  uint64_t* res_bar = bars + 2 * kC64Stages;  // [2], one per consumer warpgroup
-  float* bias_s = reinterpret_cast<float*>(bars + 16);
+  uint8_t* smem_x = smem;  // im2col: kStages activation tiles; band: p.band_slots bands
+  uint8_t* smem_w = smem + (kBand ? p.w_off : kC64Stages * kC64ActBytes);
+  uint8_t* staging = smem + (kBand ? p.staging_off : kC64Stages * kC64StageBytes);
+  const int staging_bytes = kBand ? p.staging_bytes : kC64StagingBytes;
+  const int slot_bytes = kBand ? p.slot_bytes : kC64ActBytes;
+  const bool w_resident = kBand && p.w_resident;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kC64BufferBytes);
+  uint64_t* full_bar = bars;            // [kStages]
+  uint64_t* empty_bar = bars + 8;       // [kStages]
+  uint64_t* res_bar = bars + 16;        // [2], one per consumer warpgroup
+  uint64_t* band_full = bars + 18;      // [kC64BandSlots]
+  uint64_t* band_empty = bars + 21;     // [kC64BandSlots]
+  uint64_t* w_bar = bars + 24;          // resident weights
+  float* bias_s = reinterpret_cast<float*>(bars + 32);
 
   const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);
   const int nk = p.num_k_blocks;
@@ -610,9 +667,16 @@ conv64_wgmma_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_out) : "memory");
     if (p.has_residual) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_res) : "memory");
-    for (int i = 0; i < kC64Stages; ++i) {
+    for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 4);  // one arrive per warp of the consuming warpgroup
+    }
+    if constexpr (kBand) {
+      for (int i = 0; i < kC64BandSlots; ++i) {
+        mbar_init(&band_full[i], 1);
+        mbar_init(&band_empty[i], 4);
+      }
+      mbar_init(w_bar, 1);
     }
     mbar_init(&res_bar[0], 1);
     mbar_init(&res_bar[1], 1);
@@ -628,41 +692,86 @@ conv64_wgmma_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      const int pq = p.P * p.Q;
-      for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x) {
-        int base_w[2], base_h[2], img[2];
-        const int m0 = tile * kC64Pixels;
-        const bool second = m0 + kBlockM < p.M_total;  // a half past the last pixel is not loaded: its columns are clipped
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const int m = m0 + hh * kBlockM;
-          img[hh] = m / pq;
-          const int rem = m - img[hh] * pq;
-          const int p0 = rem / p.Q;
-          base_w[hh] = (rem - p0 * p.Q) * p.stride - p.pad_w;
-          base_h[hh] = p0 * p.stride - p.pad_h;
+      if constexpr (kBand) {
+        // per k-block (r, s, cb) in K order: the band of (r, cb) before its first tap (s = 0), then the weights
+        int slot = 0;
+        uint32_t slot_phase = 0;
+        const uint32_t band_bytes = static_cast<uint32_t>(p.band_w * p.band_rows) * 128u;
+        if (w_resident) {  // every k-block's weights once, for all of this CTA's tiles
+          mbar_expect_tx(w_bar, static_cast<uint32_t>(nk) * kC64WBytes);
+          for (int kb = 0; kb < nk; ++kb)
+            tma_load_2d(smem_w + kb * kC64WBytes, &map_w, w_bar, kb * kBlockK, 0);
         }
-        const uint32_t bytes = (second ? kC64ActBytes : kC64ActBytes / 2) + kC64WBytes;
-        int tap = 0, cb = 0;
-        for (int kb = 0; kb < nk; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          mbar_expect_tx(&full_bar[stage], bytes);
-          const int r = tap / p.S;
-          const int s = tap - r * p.S;
-          uint8_t* dst = smem_x + stage * kC64ActBytes;
-          tma_load_im2col_4d(dst, &map_x, &full_bar[stage], cb * kBlockK, base_w[0], base_h[0], img[0],
-                             static_cast<uint16_t>(s), static_cast<uint16_t>(r));
-          if (second)
-            tma_load_im2col_4d(dst + kATileBytes, &map_x, &full_bar[stage], cb * kBlockK, base_w[1], base_h[1], img[1],
-                               static_cast<uint16_t>(s), static_cast<uint16_t>(r));
-          tma_load_2d(smem_w + stage * kC64WBytes, &map_w, &full_bar[stage], kb * kBlockK, 0);
-          if (++cb == p.cblocks) {
-            cb = 0;
-            ++tap;
+        for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x) {
+          const int img = tile / p.tiles_per_img;
+          const int p0 = (tile - img * p.tiles_per_img) * p.band_rows;
+          int r = 0, s = 0, cb = 0;
+          for (int kb = 0; kb < nk; ++kb) {
+            if (s == 0) {
+              mbar_wait(&band_empty[slot], slot_phase ^ 1u);
+              mbar_expect_tx(&band_full[slot], band_bytes);
+              tma_load_4d(smem_x + slot * slot_bytes, &map_x, &band_full[slot], cb * kBlockK, -p.pad_w,
+                          p0 + r - p.pad_h, img);
+              if (++slot == p.band_slots) {
+                slot = 0;
+                slot_phase ^= 1u;
+              }
+            }
+            if (!w_resident) {
+              mbar_wait(&empty_bar[stage], phase ^ 1u);
+              mbar_expect_tx(&full_bar[stage], kC64WBytes);
+              tma_load_2d(smem_w + stage * kC64WBytes, &map_w, &full_bar[stage], kb * kBlockK, 0);
+              if (++stage == kStages) {
+                stage = 0;
+                phase ^= 1u;
+              }
+            }
+            if (++cb == p.cblocks) {
+              cb = 0;
+              if (++s == p.S) {
+                s = 0;
+                ++r;
+              }
+            }
           }
-          if (++stage == kC64Stages) {
-            stage = 0;
-            phase ^= 1u;
+        }
+      } else {
+        const int pq = p.P * p.Q;
+        for (int tile = blockIdx.x; tile < p.m_tiles; tile += gridDim.x) {
+          int base_w[2], base_h[2], img[2];
+          const int m0 = tile * kC64Pixels;
+          const bool second = m0 + kBlockM < p.M_total;  // a half past the last pixel is not loaded: its columns are clipped
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int m = m0 + hh * kBlockM;
+            img[hh] = m / pq;
+            const int rem = m - img[hh] * pq;
+            const int p0 = rem / p.Q;
+            base_w[hh] = (rem - p0 * p.Q) * p.stride - p.pad_w;
+            base_h[hh] = p0 * p.stride - p.pad_h;
+          }
+          const uint32_t bytes = (second ? kC64ActBytes : kC64ActBytes / 2) + kC64WBytes;
+          int tap = 0, cb = 0;
+          for (int kb = 0; kb < nk; ++kb) {
+            mbar_wait(&empty_bar[stage], phase ^ 1u);
+            mbar_expect_tx(&full_bar[stage], bytes);
+            const int r = tap / p.S;
+            const int s = tap - r * p.S;
+            uint8_t* dst = smem_x + stage * kC64ActBytes;
+            tma_load_im2col_4d(dst, &map_x, &full_bar[stage], cb * kBlockK, base_w[0], base_h[0], img[0],
+                               static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+            if (second)
+              tma_load_im2col_4d(dst + kATileBytes, &map_x, &full_bar[stage], cb * kBlockK, base_w[1], base_h[1], img[1],
+                                 static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+            tma_load_2d(smem_w + stage * kC64WBytes, &map_w, &full_bar[stage], kb * kBlockK, 0);
+            if (++cb == p.cblocks) {
+              cb = 0;
+              ++tap;
+            }
+            if (++stage == kStages) {
+              stage = 0;
+              phase ^= 1u;
+            }
           }
         }
       }
@@ -674,94 +783,154 @@ conv64_wgmma_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
     const int t = threadIdx.x & 127;
     const int lane = threadIdx.x & 31;
     const int q = lane >> 2;
-    // after the lane ^ 4 exchange this thread holds channels (c, c + 1) + 8 h of pixel 8 j + px
+    // after the lane ^ 4 exchange this thread holds channels (c, c + 1) + 8 h of pixel column 8 j + px
     const int c = 16 * (t >> 5) + (q & ~1);
     const int px = 2 * (lane & 3) + (q & 1);
     const bool odd = (q & 1) != 0;
-    uint8_t* stage_buf = staging + cw * kC64StagingBytes;
+    uint8_t* stage_buf = staging + cw * staging_bytes;
+    if (w_resident) mbar_wait(w_bar, 0);
+    const int bands_per_tile = nk / p.S;  // R * cblocks
     int local = 0;
     for (int i = cw, tile = blockIdx.x + cw * gridDim.x; tile < p.m_tiles; i += 2, tile += 2 * gridDim.x, ++local) {
       const int m0 = tile * kC64Pixels;
+      const int img = kBand ? tile / p.tiles_per_img : 0;
+      const int p0 = kBand ? (tile - img * p.tiles_per_img) * p.band_rows : 0;
       if (p.has_residual && t == 0) {
         bulk_wait_read_all();  // the previous tile's store has read the staging tile
-        mbar_expect_tx(&res_bar[cw], kC64StagingBytes);
-        tma_load_2d(stage_buf, &map_res, &res_bar[cw], 0, m0);
+        if constexpr (kBand) {
+          mbar_expect_tx(&res_bar[cw], static_cast<uint32_t>(p.band_rows * p.Q) * 128u);
+          tma_load_4d(stage_buf, &map_res, &res_bar[cw], 0, 0, p0, img);
+        } else {
+          mbar_expect_tx(&res_bar[cw], kC64StagingBytes);
+          tma_load_2d(stage_buf, &map_res, &res_bar[cw], 0, m0);
+        }
       }
       // stage / phase from the CTA's k-block counter (both warpgroups' tiles, in tile order); unsigned, since only the
-      // counter modulo 2 * kC64Stages matters and that survives wrap-around at 2^32
+      // counter modulo 2 * kStages matters and that survives wrap-around at 2^32.  The band ring's slot and phase come
+      // from the CTA's band counter the same way (64-bit: 3 slots do not divide 2^32).
       const uint32_t g = static_cast<uint32_t>(i) * static_cast<uint32_t>(nk);
-      int stage = static_cast<int>(g % kC64Stages);
-      uint32_t phase = (g / kC64Stages) & 1u;
-      float acc[128];
+      int stage = static_cast<int>(g % kStages);
+      uint32_t phase = (g / kStages) & 1u;
+      const uint64_t gb0 = static_cast<uint64_t>(i) * static_cast<uint64_t>(bands_per_tile);
+      const int slot0 = kBand ? static_cast<int>(gb0 % static_cast<uint64_t>(p.band_slots)) : 0;
+      const uint32_t slot_phase0 = kBand ? static_cast<uint32_t>(gb0 / static_cast<uint64_t>(p.band_slots)) & 1u : 0u;
+      float acc[kN / 2];
 #pragma unroll
-      for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+      for (int j = 0; j < kN / 2; ++j) acc[j] = 0.f;
       // The mainloops take turns: this one starts once the other warpgroup has waited on every full barrier of the
       // previous tile, so no waiter is ever more than one phase behind a barrier (parity waits cannot tell phases 0 and 2
       // apart).  One arrive per following tile, so no arrival is left pending at exit.
       if (i > 0) mainloop_turn_wait(cw);
-      int prev_stage = -1;
-      auto kblock = [&](uint32_t live) {
-        mbar_wait(&full_bar[stage], phase);
-        wgmma_kblock(live, acc, make_sw128_desc(smem_u32(smem_w + stage * kC64WBytes)),
-                     make_sw128_desc(smem_u32(smem_x + stage * kC64ActBytes)));
-        wgmma_wait<1>();
-        if (prev_stage >= 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      int prev_stage = -1, prev_slot = -1;
+      // k-block (r, s, cb); the band producer's B operand is (r, cb)'s band shifted by s pixel rows
+      auto kblock = [&](uint32_t live, int kb, int r, int s, int cb) {
+        uint64_t db;
+        int slot = -1;
+        if constexpr (kBand) {
+          const int u = slot0 + r * p.cblocks + cb;  // band r * cblocks + cb of the tile
+          slot = u % p.band_slots;
+          if (s == 0) mbar_wait(&band_full[slot], slot_phase0 ^ (static_cast<uint32_t>(u / p.band_slots) & 1u));
+          db = make_sw128_desc(smem_u32(smem_x + slot * slot_bytes) + static_cast<uint32_t>(s) * 128u);
+        } else {
+          db = make_sw128_desc(smem_u32(smem_x + stage * kC64ActBytes));
         }
-        prev_stage = stage;
-        if (++stage == kC64Stages) {
-          stage = 0;
-          phase ^= 1u;
+        uint32_t wa;
+        if (w_resident) {
+          wa = smem_u32(smem_w + kb * kC64WBytes);
+        } else {
+          mbar_wait(&full_bar[stage], phase);
+          wa = smem_u32(smem_w + stage * kC64WBytes);
+        }
+        wgmma_kblock<kN>(live, acc, make_sw128_desc(wa), db);
+        wgmma_wait<1>();  // the previous k-block's MMAs have retired: its weights (and a band it used last) can go
+        __syncwarp();
+        if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+        if (prev_slot >= 0 && lane == 0) mbar_arrive(&band_empty[prev_slot]);
+        prev_slot = (kBand && s == p.S - 1) ? slot : -1;
+        if (!w_resident) {
+          prev_stage = stage;
+          if (++stage == kStages) {
+            stage = 0;
+            phase ^= 1u;
+          }
         }
       };
       if constexpr (kStemCblocks > 0) {
 #pragma unroll
-        for (int kb = 0; kb < 16 * kStemCblocks; ++kb) kblock(stem_live_steps(kb, kStemCblocks, 4));
+        for (int kb = 0; kb < 16 * kStemCblocks; ++kb)
+          kblock(stem_live_steps(kb, kStemCblocks, 4), kb, kb / (4 * kStemCblocks), (kb / kStemCblocks) % 4,
+                 kb % kStemCblocks);
       } else {
+        int r = 0, s = 0, cb = 0;
 #pragma unroll 1
-        for (int kb = 0; kb < nk; ++kb) kblock(0xFu);
+        for (int kb = 0; kb < nk; ++kb) {
+          kblock(0xFu, kb, r, s, cb);
+          if (++cb == p.cblocks) {
+            cb = 0;
+            if (++s == p.S) {
+              s = 0;
+              ++r;
+            }
+          }
+        }
       }
       if (tile + static_cast<int>(gridDim.x) < p.m_tiles) mainloop_turn_pass(cw);
       wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      if (lane == 0) {
+        if (prev_stage >= 0) mbar_arrive(&empty_bar[prev_stage]);
+        if (prev_slot >= 0) mbar_arrive(&band_empty[prev_slot]);
+      }
 
       if (t == 0) bulk_wait_read_all();
       warpgroup_sync(cw);
       if (p.has_residual) mbar_wait(&res_bar[cw], static_cast<uint32_t>(local) & 1u);
       const uint32_t sbase = smem_u32(stage_buf);
+      const float2 bias2[2] = {*reinterpret_cast<const float2*>(bias_s + c), *reinterpret_cast<const float2*>(bias_s + c + 8)};
+      // band tiles: column n = 8 j + px is output pixel (row, col) = (n / Wp, n % Wp) of the tile, staged at row * Q + col
+      // when col < Q and row < the tile's rows; im2col tiles stage column n at n
+      const int rows = kBand ? min(p.band_rows, p.P - p0) : 0;
+      int prow = 0, pcol = px;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float2 b = *reinterpret_cast<const float2*>(bias_s + c + 8 * h);
-        const int chunk = (c + 8 * h) >> 3;
+      for (int j = 0; j < kN / 8; ++j) {
+        if constexpr (kBand) {
+          while (pcol >= p.band_w) {  // Wp may be below 8
+            pcol -= p.band_w;
+            ++prow;
+          }
+        }
+        const bool keep = !kBand || (pcol < p.Q && prow < rows);
+        const int srow = kBand ? prow * p.Q + pcol : 8 * j + px;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
+        for (int h = 0; h < 2; ++h) {
           const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
           const float other = __shfl_xor_sync(0xffffffffu, odd ? v0 : v1, 4);
-          float f0 = (odd ? other : v0) + b.x;
-          float f1 = (odd ? v1 : other) + b.y;
-          const int row = 8 * j + px;  // row & 7 == px
-          const uint32_t addr =
-              sbase + static_cast<uint32_t>(row * 128 + ((chunk ^ px) << 4) + ((c & 7) << 1));
-          if (p.has_residual) {
-            uint32_t rr;
-            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rr) : "r"(addr) : "memory");
-            const float2 r = unpack_act2(rr);
-            f0 += r.x;
-            f1 += r.y;
+          float f0 = (odd ? other : v0) + bias2[h].x;
+          float f1 = (odd ? v1 : other) + bias2[h].y;
+          const int chunk = (c + 8 * h) >> 3;
+          const uint32_t addr = sbase + static_cast<uint32_t>(srow * 128 + ((chunk ^ (srow & 7)) << 4) + ((c & 7) << 1));
+          if (keep) {
+            if (p.has_residual) {
+              uint32_t rr;
+              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rr) : "r"(addr) : "memory");
+              const float2 r = unpack_act2(rr);
+              f0 += r.x;
+              f1 += r.y;
+            }
+            if (p.relu) {
+              f0 = fmaxf(f0, 0.f);
+              f1 = fmaxf(f1, 0.f);
+            }
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_act2(f0, f1)) : "memory");
           }
-          if (p.relu) {
-            f0 = fmaxf(f0, 0.f);
-            f1 = fmaxf(f1, 0.f);
-          }
-          asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_act2(f0, f1)) : "memory");
         }
+        pcol += 8;
       }
       fence_proxy_async_smem();
       warpgroup_sync(cw);
       if (t == 0) {
-        tma_store_2d(&map_out, stage_buf, 0, m0);
+        if constexpr (kBand) tma_store_4d(&map_out, stage_buf, 0, 0, p0, img);
+        else tma_store_2d(&map_out, stage_buf, 0, m0);
         bulk_commit();
       }
     }
@@ -873,19 +1042,64 @@ static int encode_2d_map(CUtensorMap* map, const void* ptr, cuuint64_t cols, cuu
   return MPX_OK;
 }
 
-static int conv64_forward(const ConvDesc& d, const CUtensorMap& map_x, const void* w, const float* bias,
-                          const void* residual, void* out, int M_total, int P, int Q, int cap, cudaStream_t stream) {
-  const int K_total = d.R * d.S * d.C_in;
-  CUtensorMap map_w, map_res, map_out;
-  int rc = encode_2d_map(&map_w, w, K_total, 64, kBlockK, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
-  if (rc != MPX_OK) return rc;
-  rc = encode_2d_map(&map_out, out, 64, M_total, 64, kC64Pixels, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
-  if (rc != MPX_OK) return rc;
-  map_res = map_out;
-  if (residual != nullptr) {
-    rc = encode_2d_map(&map_res, residual, 64, M_total, 64, kC64Pixels, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
-    if (rc != MPX_OK) return rc;
+// [n, H, W, C] act16 tensor, (64 x box_w x box_h x 1) boxes, 128B swizzle; out-of-range elements are zero-filled on load
+// and clipped on store
+static int encode_nhwc_map(CUtensorMap* map, const void* ptr, int n, int H, int W, int C, int box_w, int box_h) {
+  cuuint64_t dims[4] = {static_cast<cuuint64_t>(C), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H),
+                        static_cast<cuuint64_t>(n)};
+  cuuint64_t strides[3] = {static_cast<cuuint64_t>(C) * 2, static_cast<cuuint64_t>(W) * C * 2,
+                           static_cast<cuuint64_t>(H) * W * C * 2};
+  cuuint32_t box[4] = {static_cast<cuuint32_t>(kBlockK), static_cast<cuuint32_t>(box_w), static_cast<cuuint32_t>(box_h),
+                       1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = g_encode_tiled(map, kTmaActType, 4, const_cast<void*>(ptr), dims, strides, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  MPX_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
+  return MPX_OK;
+}
+
+// The band producer serves stride 1 when one padded input row (Wp = W + both pads = Q + S - 1 pixels) fits a TMA box
+// dimension and a ring slot, and a tile's cblocks bands leave a slot free for the producer to run ahead.
+static bool conv64_band_fits(const ConvDesc& d) {
+  const int wp = d.W + d.pad_lo_w + d.pad_hi_w;
+  return d.stride == 1 && wp <= kC64Pixels && d.C_in / kBlockK <= kC64BandSlots - 1;
+}
+
+// Shared-memory layout of the band producer.  Every tile reuses the same weights, so when all k-blocks fit beside at least
+// cblocks + 1 band slots and the two staging tiles (each sized to the tile), they are loaded once per CTA and stay
+// resident: the stem's 128 KB and layer1's 72 KB would otherwise be refetched from L2 for every tile, more bytes than its
+// bands.  Otherwise the weights go through a ring of 8 stages beside 3 slots of 32 KB.  A tap's B operand may read up to
+// (N + S - 2) pixels past its slot's start for columns that are dropped; those reads must stay inside the layout.
+static void conv64_band_layout(Conv64Params& p, int band_n, int S) {
+  auto round1k = [](int b) { return (b + 1023) & ~1023; };
+  const int slot = round1k(p.band_w * p.band_rows * 128);
+  const int staging = round1k(p.band_rows * p.Q * 128);
+  const int weights = p.num_k_blocks * kC64WBytes;
+  const int reach = (band_n + S - 2) * 128 + 128;
+  for (int slots = kC64BandSlots; slots >= p.cblocks + 1; --slots) {
+    const int end = slots * slot + weights + 2 * staging;
+    if (end <= kC64BufferBytes && (slots - 1) * slot + reach <= kC64BufferBytes) {
+      p.band_slots = slots;
+      p.slot_bytes = slot;
+      p.w_resident = 1;
+      p.w_off = slots * slot;
+      p.staging_off = p.w_off + weights;
+      p.staging_bytes = staging;
+      return;
+    }
   }
+  p.band_slots = kC64BandSlots;
+  p.slot_bytes = kC64ActBytes;
+  p.w_resident = 0;
+  p.w_off = kC64BandSlots * kC64ActBytes;
+  p.staging_off = p.w_off + kC64BandWStages * kC64WBytes;
+  p.staging_bytes = kC64StagingBytes;
+}
+
+static int conv64_forward(const ConvDesc& d, const void* x, const void* w, const float* bias, const void* residual,
+                          void* out, int M_total, int P, int Q, int cap, cudaStream_t stream) {
+  const int K_total = d.R * d.S * d.C_in;
   Conv64Params p{};
   p.M_total = M_total;
   p.P = P;
@@ -896,30 +1110,67 @@ static int conv64_forward(const ConvDesc& d, const CUtensorMap& map_x, const voi
   p.pad_w = d.pad_lo_w;
   p.cblocks = d.C_in / kBlockK;
   p.num_k_blocks = d.R * d.S * p.cblocks;
-  p.m_tiles = (M_total + kC64Pixels - 1) / kC64Pixels;
   p.relu = d.relu;
   p.has_residual = residual != nullptr;
   p.bias = bias;
+  // mode bit 23 keeps every shape on the im2col producer
+  const bool band = conv64_band_fits(d) && (g_conv_mode & 8388608) == 0;
+  int band_n = 0;
+  CUtensorMap map_x, map_w, map_res, map_out;
+  int rc;
+  if (band) {
+    p.band_w = d.W + d.pad_lo_w + d.pad_hi_w;
+    p.band_rows = kC64Pixels / p.band_w < P ? kC64Pixels / p.band_w : P;
+    p.tiles_per_img = (P + p.band_rows - 1) / p.band_rows;
+    p.m_tiles = d.n_img * p.tiles_per_img;
+    // the columns a tile's MMAs must cover: its last row ends (band_rows - 1) * Wp + Q columns in
+    band_n = (p.band_rows - 1) * p.band_w + Q <= 160 ? 160 : 256;
+    conv64_band_layout(p, band_n, d.S);
+    rc = encode_nhwc_map(&map_x, x, d.n_img, d.H, d.W, d.C_in, p.band_w, p.band_rows);
+    if (rc != MPX_OK) return rc;
+    rc = encode_nhwc_map(&map_out, out, d.n_img, P, Q, 64, Q, p.band_rows);
+    if (rc != MPX_OK) return rc;
+    map_res = map_out;
+    if (residual != nullptr) {
+      rc = encode_nhwc_map(&map_res, residual, d.n_img, P, Q, 64, Q, p.band_rows);
+      if (rc != MPX_OK) return rc;
+    }
+  } else {
+    p.m_tiles = (M_total + kC64Pixels - 1) / kC64Pixels;
+    rc = encode_im2col_map(&map_x, d, x);
+    if (rc != MPX_OK) return rc;
+    rc = encode_2d_map(&map_out, out, 64, M_total, 64, kC64Pixels, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+    if (rc != MPX_OK) return rc;
+    map_res = map_out;
+    if (residual != nullptr) {
+      rc = encode_2d_map(&map_res, residual, 64, M_total, 64, kC64Pixels, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+      if (rc != MPX_OK) return rc;
+    }
+  }
+  rc = encode_2d_map(&map_w, w, K_total, 64, kBlockK, 64, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  if (rc != MPX_OK) return rc;
   // the coarse / scoring (c_pad 16) and refiner (c_pad 32) stems skip their zero slices; wider c_pad issues every step
   const int stem_cblocks = (d.s2d_stem && d.R == 4 && d.S == 4 && p.cblocks <= 2) ? p.cblocks : 0;
-  long long live_steps = 0;  // k16 steps issued per tile
+  long long live_steps = 0;  // k16 steps per tile
   for (int kb = 0; kb < p.num_k_blocks; ++kb)
     live_steps += __builtin_popcount(stem_cblocks ? stem_live_steps(kb, p.cblocks, p.S) : 0xFu);
 
+  typedef void (*Conv64Kernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, Conv64Params);
+  // [stem cblocks][im2col, band n160, band n256]
+  static const Conv64Kernel kernels[3][3] = {
+      {conv64_wgmma_kernel<0, 0>, conv64_wgmma_kernel<0, 160>, conv64_wgmma_kernel<0, 256>},
+      {conv64_wgmma_kernel<1, 0>, conv64_wgmma_kernel<1, 160>, conv64_wgmma_kernel<1, 256>},
+      {conv64_wgmma_kernel<2, 0>, conv64_wgmma_kernel<2, 160>, conv64_wgmma_kernel<2, 256>}};
   static bool attr_set = false;
   if (!attr_set) {
-    MPX_CHECK_CUDA(cudaFuncSetAttribute(conv64_wgmma_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        kC64SmemBytes));
-    MPX_CHECK_CUDA(cudaFuncSetAttribute(conv64_wgmma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        kC64SmemBytes));
-    MPX_CHECK_CUDA(cudaFuncSetAttribute(conv64_wgmma_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        kC64SmemBytes));
+    for (int a = 0; a < 3; ++a)
+      for (int b = 0; b < 3; ++b)
+        MPX_CHECK_CUDA(cudaFuncSetAttribute(kernels[a][b], cudaFuncAttributeMaxDynamicSharedMemorySize, kC64SmemBytes));
     attr_set = true;
   }
   const int grid = p.m_tiles < cap ? p.m_tiles : cap;
   ProfileSlot* slot = profile_begin(stream);
-  void (*kernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, Conv64Params) =
-      stem_cblocks == 1 ? conv64_wgmma_kernel<1> : (stem_cblocks == 2 ? conv64_wgmma_kernel<2> : conv64_wgmma_kernel<0>);
+  const Conv64Kernel kernel = kernels[stem_cblocks][band_n == 0 ? 0 : (band_n == 160 ? 1 : 2)];
   MPX_CHECK_CUDA(launch_pdl(kernel, dim3(grid), dim3(kThreads), kC64SmemBytes, stream, 1, map_x, map_w, map_res, map_out,
                             p));
   MPX_CHECK_CUDA(cudaGetLastError());
@@ -960,13 +1211,9 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
   MPX_REQUIRE((block_n == 64 || block_n == 128 || block_n == 256) && d.C_out % block_n == 0,
               "conv: BLOCK_N=%d invalid for C_out=%d", block_n, d.C_out);
 
-  // --- activation map (im2col): 128-pixel boxes of 64 channels
-  CUtensorMap map_a, map_b;
-  rc = encode_im2col_map(&map_a, d, x);
-  if (rc != MPX_OK) return rc;
-
   // C_out = 64 with enough 256-pixel tiles to give every CTA at least two (one per consumer warpgroup): the pixel-major
-  // kernel.  Mode bit 22 never takes it, bit 26 takes it whatever the size.
+  // kernel.  Mode bit 22 never takes it, bit 26 takes it whatever the size.  It loads its activations by filter-row band
+  // where conv64_band_fits, by im2col otherwise (or under bit 23).
   const bool aligned = (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(residual) & 15) == 0;
   const long long tiles256 = (M_total + kC64Pixels - 1) / kC64Pixels;
   const int cap = max_ctas > 0 ? max_ctas : sm_count();
@@ -977,9 +1224,13 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
     const long long m_tiles128 = (M_total + kBlockM - 1) / kBlockM;
     const int nkb = d.R * d.S * (d.C_in / kBlockK);
     if (!(splitk < 0 && m_tiles128 * 2 <= cap && nkb >= 8))
-      return conv64_forward(d, map_a, w, bias, residual, out, static_cast<int>(M_total), P, Q, cap, stream);
+      return conv64_forward(d, x, w, bias, residual, out, static_cast<int>(M_total), P, Q, cap, stream);
   }
 
+  // --- activation map (im2col): 128-pixel boxes of 64 channels
+  CUtensorMap map_a, map_b;
+  rc = encode_im2col_map(&map_a, d, x);
+  if (rc != MPX_OK) return rc;
   rc = encode_2d_map(&map_b, w, static_cast<cuuint64_t>(d.R) * d.S * d.C_in, d.C_out, kBlockK, block_n,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (rc != MPX_OK) return rc;
