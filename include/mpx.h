@@ -340,6 +340,68 @@ int mpx_bop_point_errors(int kind, int n_pairs, int n_models, const double* d_pt
                          const int32_t* d_model_idx, const double* d_pose_est, const double* d_pose_gt, const double* d_K,
                          double* d_err, int32_t* d_sym_argmin, void* stream);
 
+/* ---- depth refinement (TEASER++) ----------------------------------------------------------------------------------
+ * Replaces the per-prediction host path of TeaserppRefiner.refine_poses / compute_teaserpp_refinement
+ * (inference/teaserpp_refiner.py:53-161, 208-287): meshcat_utils.get_pointcloud, refiner_utils.compute_masks,
+ * pytorch3d.ops.sample_farthest_points and teaserpp_python.RobustRegistrationSolver (known correspondences, no scale,
+ * GNC-TLS rotation, PMC_EXACT max clique).  megapose6d_b200/teaserpp_refiner.py drives the stages; each is ONE launch for
+ * all n_pred predictions of a call.  The arithmetic is the contract stated in DESIGN §4 (parity with the libraries is not
+ * pinned).  Sizes: n_pred >= 0, h, w > 0 with h * w < 2^31, 1 <= k <= MPX_TEASER_MAX_POINTS.  Refused before any launch:
+ * bad sizes, a NULL required pointer, a required pointer that is not device memory.
+ *
+ * mpx_teaser_points: prediction p compares d_depth_rendered[p] [n_pred, h, w] with d_depth_measured[d_view_idx[p]]
+ * [n_view, h, w] (float32 metres) under d_K[p] [n_pred, 9] float32.  mask_type MPX_TEASER_MASK_SIMPLE (both depths > 0) or
+ * MPX_TEASER_MASK_THRESHOLD (also |measured - rendered| <= thresh).  Masked pixels in row-major order go to
+ * d_src / d_tgt [n_pred, h * w, 3] float32 (x = fp32((u - cx) * fp32(z / fx)) in float64, likewise y; z), d_count [n_pred]
+ * int32 receives the number of masked pixels.  d_raw_src / d_raw_tgt [n_pred, h, w, 3] (may be NULL) receive the
+ * unmasked clouds. */
+#define MPX_TEASER_MAX_POINTS 1024
+#define MPX_TEASER_MASK_SIMPLE 0
+#define MPX_TEASER_MASK_THRESHOLD 1
+int mpx_teaser_points(int n_pred, int h, int w, const float* d_depth_rendered, const float* d_depth_measured, int n_view,
+                      const int32_t* d_view_idx, const float* d_K, int mask_type, float thresh, float* d_src, float* d_tgt,
+                      int32_t* d_count, float* d_raw_src, float* d_raw_tgt, void* stream);
+
+/* mpx_teaser_fps: farthest-point sampling of the n = min(d_count[p], cap) points of d_src[p] [n_pred, cap, 3] (one
+ * 8-CTA cluster per prediction): index 0, then k - 1 times the arg-max (lowest index on ties) of the running minimum of
+ * the fp32 squared distances dx*dx + dy*dy + dz*dz; for n < k the remaining indices are n - 1.  d_idx [n_pred, k] int32
+ * (-1 when n == 0); d_samp_src / d_samp_tgt [n_pred, k, 3] float32 receive d_src / d_tgt at those indices (zeros when
+ * n == 0).  d_workspace: mpx_teaser_fps_workspace_bytes(n_pred, cap) bytes. */
+size_t mpx_teaser_fps_workspace_bytes(int n_pred, int cap);
+int mpx_teaser_fps(int n_pred, int cap, const float* d_src, const float* d_tgt, const int32_t* d_count, int k,
+                   int32_t* d_idx, float* d_samp_src, float* d_samp_tgt, void* d_workspace, size_t workspace_bytes,
+                   void* stream);
+
+/* mpx_teaser_graph: consistency graph of the d_m[p] (0..k) samples of prediction p (d_samp_src / d_samp_tgt
+ * [n_pred, k, 3] float32): d_adj [n_pred, k, 16] uint64, bit j % 64 of word j / 64 of row i set when i != j and
+ * | ||t_j - t_i|| - ||s_j - s_i|| | <= bound, in float64 without contraction (norm = sqrt((x*x + y*y) + z*z)). */
+int mpx_teaser_graph(int n_pred, int k, const float* d_samp_src, const float* d_samp_tgt, const int32_t* d_m, double bound,
+                     uint64_t* d_adj, void* stream);
+
+/* mpx_teaser_max_clique: maximum clique of each graph (one CTA per prediction): core numbers by peeling, a greedy clique in
+ * core order, then branch and bound with a greedy-colouring bound.  The search expands at most node_budget nodes
+ * (<= 0: MPX_TEASER_CLIQUE_NODE_BUDGET); when the budget runs out the best clique found so far is returned and bit 0 of
+ * d_status[p] is set.  d_clique [n_pred, k] int32: the clique's vertices in ascending order (then -1), d_clique_size
+ * [n_pred] int32, d_status [n_pred] int32 (bit 0: budget exhausted), d_nodes [n_pred] int64 (may be NULL): nodes
+ * expanded.  d_workspace: mpx_teaser_clique_workspace_bytes(n_pred, k) bytes. */
+#define MPX_TEASER_CLIQUE_NODE_BUDGET 20000
+size_t mpx_teaser_clique_workspace_bytes(int n_pred, int k);
+int mpx_teaser_max_clique(int n_pred, int k, const uint64_t* d_adj, const int32_t* d_m, long long node_budget,
+                          int32_t* d_clique, int32_t* d_clique_size, int32_t* d_status, int64_t* d_nodes,
+                          void* d_workspace, size_t workspace_bytes, void* stream);
+
+/* mpx_teaser_solve: for every prediction whose clique has >= 2 vertices: GNC-TLS rotation on the chain TIMs of the clique
+ * (TIM bound 2 noise_bound, factor gnc_factor, at most max_iterations, stop on |cost change| < cost_threshold; weighted
+ * Kabsch by a float64 Jacobi SVD), per-axis adaptive-voting TLS translation (bound noise_bound), the number of the d_m[p]
+ * samples with ||R s + t - t_i|| < noise_bound.  Outputs: d_T [n_pred, 16] float64 (row-major 4x4; identity when the
+ * clique is invalid), d_num_inliers [n_pred] int32, d_flags [n_pred] int32 (bit 0 valid, bit 1 accepted).  Accepted
+ * (valid and num_inliers >= min_num_inliers): d_poses_input[p] = d_poses[p], then d_poses[p] = fp32(T @ double(d_poses[p]))
+ * ([n_pred, 16] float32, updated in place). */
+int mpx_teaser_solve(int n_pred, int k, const float* d_samp_src, const float* d_samp_tgt, const int32_t* d_m,
+                     const int32_t* d_clique, const int32_t* d_clique_size, double noise_bound, double gnc_factor,
+                     int max_iterations, double cost_threshold, int min_num_inliers, float* d_poses, float* d_poses_input,
+                     double* d_T, int32_t* d_num_inliers, int32_t* d_flags, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

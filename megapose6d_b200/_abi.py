@@ -72,6 +72,16 @@ def _declare(lib: ctypes.CDLL) -> None:
                                 c_float, vp, vp, vp]
     lib.mpx_bop_point_errors.argtypes = [c_int, c_int, c_int, vp, vp, ctypes.c_longlong, vp, vp, ctypes.c_longlong, vp, vp,
                                          vp, vp, vp, vp, vp]
+    lib.mpx_teaser_points.argtypes = [c_int, c_int, c_int, vp, vp, c_int, vp, vp, c_int, c_float, vp, vp, vp, vp, vp, vp]
+    lib.mpx_teaser_fps_workspace_bytes.argtypes = [c_int, c_int]
+    lib.mpx_teaser_fps_workspace_bytes.restype = c_size_t
+    lib.mpx_teaser_fps.argtypes = [c_int, c_int, vp, vp, vp, c_int, vp, vp, vp, vp, c_size_t, vp]
+    lib.mpx_teaser_graph.argtypes = [c_int, c_int, vp, vp, vp, ctypes.c_double, vp, vp]
+    lib.mpx_teaser_clique_workspace_bytes.argtypes = [c_int, c_int]
+    lib.mpx_teaser_clique_workspace_bytes.restype = c_size_t
+    lib.mpx_teaser_max_clique.argtypes = [c_int, c_int, vp, vp, ctypes.c_longlong, vp, vp, vp, vp, vp, c_size_t, vp]
+    lib.mpx_teaser_solve.argtypes = [c_int, c_int, vp, vp, vp, vp, vp, ctypes.c_double, ctypes.c_double, c_int,
+                                     ctypes.c_double, c_int, vp, vp, vp, vp, vp, vp]
     lib.mpx_launch_count.restype = ctypes.c_longlong
     lib.mpx_profile_enable.argtypes = [c_int]
     lib.mpx_set_sm_limit.argtypes = [c_int]
@@ -95,6 +105,8 @@ EXPORTS = [
     "mpx_net_input_bytes", "mpx_conv2d", "mpx_conv2d_splitk", "mpx_conv_set_mode", "mpx_maxpool3x3s2", "mpx_avgpool_linear",
     "mpx_net_create", "mpx_net_create_preact", "mpx_net_destroy", "mpx_net_set_graphs", "mpx_net_workspace_bytes", "mpx_net_forward",
     "mpx_bop_vsd", "mpx_bop_point_errors",
+    "mpx_teaser_points", "mpx_teaser_fps_workspace_bytes", "mpx_teaser_fps", "mpx_teaser_graph",
+    "mpx_teaser_clique_workspace_bytes", "mpx_teaser_max_clique", "mpx_teaser_solve",
 ]
 
 

@@ -504,4 +504,132 @@ int mpx_bop_point_errors(int kind, int n_pairs, int n_models, const double* d_pt
                           d_model_idx, d_pose_est, d_pose_gt, d_K, d_err, d_sym_argmin, static_cast<cudaStream_t>(stream));
 }
 
+// ---- depth refinement (TEASER++) ----
+static bool is_device_ptr(const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
+}
+#define MPX_DEVICE(p)                                                                                                 \
+  do {                                                                                                                \
+    MPX_NOT_NULL(p);                                                                                                  \
+    MPX_REQUIRE(is_device_ptr(p), "%s: argument %s is not device memory", __func__, #p);                              \
+  } while (0)
+#define MPX_DEVICE_OR_NULL(p)                                                                                         \
+  do {                                                                                                                \
+    if (p) MPX_DEVICE(p);                                                                                             \
+  } while (0)
+
+int mpx_teaser_points(int n_pred, int h, int w, const float* d_depth_rendered, const float* d_depth_measured, int n_view,
+                      const int32_t* d_view_idx, const float* d_K, int mask_type, float thresh, float* d_src, float* d_tgt,
+                      int32_t* d_count, float* d_raw_src, float* d_raw_tgt, void* stream) {
+  MPX_REQUIRE(n_pred >= 0, "mpx_teaser_points: n_pred=%d < 0", n_pred);
+  MPX_REQUIRE(mask_type == MPX_TEASER_MASK_SIMPLE || mask_type == MPX_TEASER_MASK_THRESHOLD,
+              "mpx_teaser_points: unknown mask type %d", mask_type);
+  if (n_pred == 0) return MPX_OK;
+  MPX_REQUIRE(h > 0 && w > 0 && static_cast<long long>(h) * w < (1ll << 31), "mpx_teaser_points: bad image size %dx%d", h, w);
+  MPX_REQUIRE(n_view > 0, "mpx_teaser_points: n_view=%d", n_view);
+  MPX_REQUIRE((d_raw_src == nullptr) == (d_raw_tgt == nullptr), "mpx_teaser_points: give both raw clouds or neither");
+  MPX_DEVICE(d_depth_rendered);
+  MPX_DEVICE(d_depth_measured);
+  MPX_DEVICE(d_view_idx);
+  MPX_DEVICE(d_K);
+  MPX_DEVICE(d_src);
+  MPX_DEVICE(d_tgt);
+  MPX_DEVICE(d_count);
+  MPX_DEVICE_OR_NULL(d_raw_src);
+  MPX_DEVICE_OR_NULL(d_raw_tgt);
+  return teaser_points(n_pred, h, w, d_depth_rendered, d_depth_measured, d_view_idx, d_K, mask_type, thresh, d_src, d_tgt,
+                       d_count, d_raw_src, d_raw_tgt, static_cast<cudaStream_t>(stream));
+}
+
+size_t mpx_teaser_fps_workspace_bytes(int n_pred, int cap) {
+  return n_pred > 0 && cap > 0 ? teaser_fps_workspace_bytes(n_pred, cap) : 0;
+}
+
+int mpx_teaser_fps(int n_pred, int cap, const float* d_src, const float* d_tgt, const int32_t* d_count, int k,
+                   int32_t* d_idx, float* d_samp_src, float* d_samp_tgt, void* d_workspace, size_t workspace_bytes,
+                   void* stream) {
+  MPX_REQUIRE(n_pred >= 0, "mpx_teaser_fps: n_pred=%d < 0", n_pred);
+  MPX_REQUIRE(k >= 1 && k <= MPX_TEASER_MAX_POINTS, "mpx_teaser_fps: k=%d not in 1..%d", k, MPX_TEASER_MAX_POINTS);
+  if (n_pred == 0) return MPX_OK;
+  MPX_REQUIRE(cap > 0, "mpx_teaser_fps: cap=%d", cap);
+  MPX_REQUIRE(workspace_bytes >= teaser_fps_workspace_bytes(n_pred, cap), "mpx_teaser_fps: workspace of %zu bytes < %zu",
+              workspace_bytes, teaser_fps_workspace_bytes(n_pred, cap));
+  MPX_DEVICE(d_src);
+  MPX_DEVICE(d_tgt);
+  MPX_DEVICE(d_count);
+  MPX_DEVICE(d_idx);
+  MPX_DEVICE(d_samp_src);
+  MPX_DEVICE(d_samp_tgt);
+  MPX_DEVICE(d_workspace);
+  return teaser_fps(n_pred, cap, d_src, d_tgt, d_count, k, d_idx, d_samp_src, d_samp_tgt, d_workspace,
+                    static_cast<cudaStream_t>(stream));
+}
+
+int mpx_teaser_graph(int n_pred, int k, const float* d_samp_src, const float* d_samp_tgt, const int32_t* d_m, double bound,
+                     uint64_t* d_adj, void* stream) {
+  MPX_REQUIRE(n_pred >= 0, "mpx_teaser_graph: n_pred=%d < 0", n_pred);
+  MPX_REQUIRE(k >= 1 && k <= MPX_TEASER_MAX_POINTS, "mpx_teaser_graph: k=%d not in 1..%d", k, MPX_TEASER_MAX_POINTS);
+  if (n_pred == 0) return MPX_OK;
+  MPX_DEVICE(d_samp_src);
+  MPX_DEVICE(d_samp_tgt);
+  MPX_DEVICE(d_m);
+  MPX_DEVICE(d_adj);
+  return teaser_graph(n_pred, k, d_samp_src, d_samp_tgt, d_m, bound, reinterpret_cast<unsigned long long*>(d_adj),
+                      static_cast<cudaStream_t>(stream));
+}
+
+size_t mpx_teaser_clique_workspace_bytes(int n_pred, int k) {
+  return n_pred > 0 && k > 0 ? teaser_clique_workspace_bytes(n_pred, k) : 0;
+}
+
+int mpx_teaser_max_clique(int n_pred, int k, const uint64_t* d_adj, const int32_t* d_m, long long node_budget,
+                          int32_t* d_clique, int32_t* d_clique_size, int32_t* d_status, int64_t* d_nodes,
+                          void* d_workspace, size_t workspace_bytes, void* stream) {
+  MPX_REQUIRE(n_pred >= 0, "mpx_teaser_max_clique: n_pred=%d < 0", n_pred);
+  MPX_REQUIRE(k >= 1 && k <= MPX_TEASER_MAX_POINTS, "mpx_teaser_max_clique: k=%d not in 1..%d", k, MPX_TEASER_MAX_POINTS);
+  if (n_pred == 0) return MPX_OK;
+  MPX_REQUIRE(workspace_bytes >= teaser_clique_workspace_bytes(n_pred, k),
+              "mpx_teaser_max_clique: workspace of %zu bytes < %zu", workspace_bytes,
+              teaser_clique_workspace_bytes(n_pred, k));
+  MPX_DEVICE(d_adj);
+  MPX_DEVICE(d_m);
+  MPX_DEVICE(d_clique);
+  MPX_DEVICE(d_clique_size);
+  MPX_DEVICE(d_status);
+  MPX_DEVICE_OR_NULL(d_nodes);
+  MPX_DEVICE(d_workspace);
+  return teaser_max_clique(n_pred, k, reinterpret_cast<const unsigned long long*>(d_adj), d_m,
+                           node_budget > 0 ? node_budget : MPX_TEASER_CLIQUE_NODE_BUDGET, d_clique, d_clique_size,
+                           d_status, reinterpret_cast<long long*>(d_nodes), d_workspace, static_cast<cudaStream_t>(stream));
+}
+
+int mpx_teaser_solve(int n_pred, int k, const float* d_samp_src, const float* d_samp_tgt, const int32_t* d_m,
+                     const int32_t* d_clique, const int32_t* d_clique_size, double noise_bound, double gnc_factor,
+                     int max_iterations, double cost_threshold, int min_num_inliers, float* d_poses, float* d_poses_input,
+                     double* d_T, int32_t* d_num_inliers, int32_t* d_flags, void* stream) {
+  MPX_REQUIRE(n_pred >= 0, "mpx_teaser_solve: n_pred=%d < 0", n_pred);
+  MPX_REQUIRE(k >= 1 && k <= MPX_TEASER_MAX_POINTS, "mpx_teaser_solve: k=%d not in 1..%d", k, MPX_TEASER_MAX_POINTS);
+  MPX_REQUIRE(noise_bound > 0 && gnc_factor > 1 && max_iterations >= 1,
+              "mpx_teaser_solve: noise_bound=%g gnc_factor=%g max_iterations=%d", noise_bound, gnc_factor, max_iterations);
+  if (n_pred == 0) return MPX_OK;
+  MPX_DEVICE(d_samp_src);
+  MPX_DEVICE(d_samp_tgt);
+  MPX_DEVICE(d_m);
+  MPX_DEVICE(d_clique);
+  MPX_DEVICE(d_clique_size);
+  MPX_DEVICE(d_poses);
+  MPX_DEVICE(d_poses_input);
+  MPX_DEVICE(d_T);
+  MPX_DEVICE(d_num_inliers);
+  MPX_DEVICE(d_flags);
+  return teaser_solve(n_pred, k, d_samp_src, d_samp_tgt, d_m, d_clique, d_clique_size, noise_bound, gnc_factor,
+                      max_iterations, cost_threshold, min_num_inliers, d_poses, d_poses_input, d_T, d_num_inliers, d_flags,
+                      static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

@@ -298,4 +298,21 @@ int bop_point_errors(int kind, int n_pairs, int n_models, const double* pts, con
                      const double* pose_est, const double* pose_gt, const double* K, double* err, int* sym_argmin,
                      cudaStream_t stream);
 
+
+// teaser.cu
+int teaser_points(int n_pred, int h, int w, const float* rend, const float* meas, const int* view_idx, const float* K,
+                  int mask_type, float thresh, float* src, float* tgt, int* count, float* raw_src, float* raw_tgt,
+                  cudaStream_t stream);
+size_t teaser_fps_workspace_bytes(int n_pred, int cap);
+int teaser_fps(int n_pred, int cap, const float* src, const float* tgt, const int* count, int k, int* idx,
+               float* samp_src, float* samp_tgt, void* ws, cudaStream_t stream);
+int teaser_graph(int n_pred, int k, const float* ss, const float* st, const int* m, double bound,
+                 unsigned long long* adj, cudaStream_t stream);
+size_t teaser_clique_workspace_bytes(int n_pred, int k);
+int teaser_max_clique(int n_pred, int k, const unsigned long long* adj, const int* m, long long budget, int* clique,
+                      int* size, int* status, long long* nodes, void* ws, cudaStream_t stream);
+int teaser_solve(int n_pred, int k, const float* ss, const float* st, const int* m, const int* clique, const int* csize,
+                 double noise_bound, double gnc_factor, int max_it, double cost_thr, int min_inliers, float* poses,
+                 float* poses_input, double* T, int* n_in, int* flags, cudaStream_t stream);
+
 }  // namespace mpx

@@ -485,16 +485,27 @@ def main(argv: Optional[List[str]] = None) -> None:
     parser.add_argument("--models-root", type=Path, default=None)
     parser.add_argument("--meshes-from", type=Path, default=None)
     parser.add_argument("--save-dir", type=Path, required=True)
+    parser.add_argument("--depth-refiner", choices=["icp", "teaserpp"], default=None,
+                        help="refine the final poses against the frames' depth (evaluation/evaluation.py:132-139)")
     args = parser.parse_args(argv)
     if "RANK" in os.environ and not dist.is_initialized():
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", 0)))
         dist.init_process_group("nccl")
     info = NAMED_MODELS[args.model]
+    if args.depth_refiner is not None and not info["requires_depth"]:
+        parser.error(f"--depth-refiner needs a model that loads depth; {args.model} does not")
     params = info["inference_parameters"]
     cfg = InferenceConfig(detection_type="gt", n_refiner_iterations=params["n_refiner_iterations"],
-                          n_pose_hypotheses=params["n_pose_hypotheses"], run_depth_refiner=False, bsz_images=576, bsz_objects=16)
+                          n_pose_hypotheses=params["n_pose_hypotheses"], run_depth_refiner=args.depth_refiner is not None,
+                          depth_refiner=args.depth_refiner, bsz_images=576, bsz_objects=16)
     object_dataset = make_object_dataset(args.meshes_from or args.frame_dirs[0])
     pose_estimator = load_named_model(args.model, object_dataset, models_root=args.models_root).cuda()
+    if args.depth_refiner is not None:
+        from .icp_refiner import ICPRefiner
+        from .teaserpp_refiner import TeaserppRefiner
+
+        cls = ICPRefiner if args.depth_refiner == "icp" else TeaserppRefiner
+        pose_estimator.depth_refiner = cls(pose_estimator.refiner_model.mesh_db, pose_estimator.refiner_model.renderer)
     scene_ds = ExampleDirSceneDataset(args.frame_dirs, load_depth=info["requires_depth"])
     out = run_predictions(scene_ds, pose_estimator, cfg, save_dir=args.save_dir)
     if out["save_dir"] is not None:
