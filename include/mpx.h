@@ -340,6 +340,24 @@ int mpx_bop_point_errors(int kind, int n_pairs, int n_models, const double* d_pt
                          const int32_t* d_model_idx, const double* d_pose_est, const double* d_pose_gt, const double* d_K,
                          double* d_err, int32_t* d_sym_argmin, void* stream);
 
+/* mpx_bop_gt_info: the per-gt outputs of the toolkit's scripts/calc_gt_info.py and scripts/calc_gt_masks.py (which the
+ * reference's BOPDataset reads as scene_gt_info.json and mask_visib/) for n_gt ground-truth instances of any number of test
+ * images, in one pass.  Gt g lies in image i = d_img_idx[g] (d_depth_test [n_img, h, w] raw uint16, d_depth_scale [n_img],
+ * d_K [n_img, 9] float64, as mpx_bop_vsd); d_depth_gt_large [n_gt, 3h, 3w] float32 METRES (0 = no surface) is its render
+ * alone on the scripts' enlarged canvas, principal point shifted by (w, h), so that the image is the window at (w, h).
+ * Depth in mm and the scene_gt_info arithmetic (depth_im_to_dist_im_fast, bop19 visibility against delta in mm) are those
+ * of mpx_bop_vsd.  Outputs: d_counts [n_gt, 3] int64 = {px_count_all (canvas), px_count_valid, px_count_visib (image)};
+ * d_bbox [n_gt, 8] int32 = {bbox_obj, bbox_visib} as misc.calc_2d_bbox (x, y, x_max - x_min, y_max - y_min), in image
+ * coordinates (bbox_obj may be negative), both [-1, -1, -1, -1] unless px_count_visib > 0; d_mask / d_mask_visib
+ * [n_gt, h, w] uint8 0/1 (either may be NULL) = calc_gt_masks.py's model-distance > 0 and bop19 visibility, whose distance
+ * images come from misc.depth_im_to_dist_im (X d = ((x - cx) d) (1 / fx)): near delta, mask_visib can differ from the
+ * visibility that px_count_visib counts.  A gt whose image index is out of range gets counts and boxes of -1 and empty masks.
+ * The counts and boxes are integer reductions: they do not depend on the launch shape.  Refused before any launch:
+ * n_gt < 0, n_img < 1, empty images, 9 h w >= 2^31, a NULL or non-device required pointer, non-device masks. */
+int mpx_bop_gt_info(int n_gt, int h, int w, const uint16_t* d_depth_test, int n_img, const float* d_depth_scale,
+                    const double* d_K, const float* d_depth_gt_large, const int32_t* d_img_idx, float delta,
+                    int64_t* d_counts, int32_t* d_bbox, uint8_t* d_mask, uint8_t* d_mask_visib, void* stream);
+
 /* ---- depth refinement (TEASER++) ----------------------------------------------------------------------------------
  * Replaces the per-prediction host path of TeaserppRefiner.refine_poses / compute_teaserpp_refinement
  * (inference/teaserpp_refiner.py:53-161, 208-287): meshcat_utils.get_pointcloud, refiner_utils.compute_masks,

@@ -72,6 +72,7 @@ def _declare(lib: ctypes.CDLL) -> None:
                                 c_float, vp, vp, vp]
     lib.mpx_bop_point_errors.argtypes = [c_int, c_int, c_int, vp, vp, ctypes.c_longlong, vp, vp, ctypes.c_longlong, vp, vp,
                                          vp, vp, vp, vp, vp]
+    lib.mpx_bop_gt_info.argtypes = [c_int, c_int, c_int, vp, c_int, vp, vp, vp, vp, c_float, vp, vp, vp, vp, vp]
     lib.mpx_teaser_points.argtypes = [c_int, c_int, c_int, vp, vp, c_int, vp, vp, c_int, c_float, vp, vp, vp, vp, vp, vp]
     lib.mpx_teaser_fps_workspace_bytes.argtypes = [c_int, c_int]
     lib.mpx_teaser_fps_workspace_bytes.restype = c_size_t
@@ -104,7 +105,7 @@ EXPORTS = [
     "mpx_pose_update", "mpx_topk_per_group", "mpx_image_to_nhwc4", "mpx_roi_align", "mpx_roi_align_fused",
     "mpx_net_input_bytes", "mpx_conv2d", "mpx_conv2d_splitk", "mpx_conv_set_mode", "mpx_maxpool3x3s2", "mpx_avgpool_linear",
     "mpx_net_create", "mpx_net_create_preact", "mpx_net_destroy", "mpx_net_set_graphs", "mpx_net_workspace_bytes", "mpx_net_forward",
-    "mpx_bop_vsd", "mpx_bop_point_errors",
+    "mpx_bop_vsd", "mpx_bop_point_errors", "mpx_bop_gt_info",
     "mpx_teaser_points", "mpx_teaser_fps_workspace_bytes", "mpx_teaser_fps", "mpx_teaser_graph",
     "mpx_teaser_clique_workspace_bytes", "mpx_teaser_max_clique", "mpx_teaser_solve",
 ]

@@ -632,4 +632,25 @@ int mpx_teaser_solve(int n_pred, int k, const float* d_samp_src, const float* d_
                       static_cast<cudaStream_t>(stream));
 }
 
+// ---- BOP ground-truth annotation (a BOP 2019 group entry point, placed here for the device-pointer checks) ----
+int mpx_bop_gt_info(int n_gt, int h, int w, const uint16_t* d_depth_test, int n_img, const float* d_depth_scale,
+                    const double* d_K, const float* d_depth_gt_large, const int32_t* d_img_idx, float delta,
+                    int64_t* d_counts, int32_t* d_bbox, uint8_t* d_mask, uint8_t* d_mask_visib, void* stream) {
+  MPX_REQUIRE(n_gt >= 0, "mpx_bop_gt_info: n_gt=%d < 0", n_gt);
+  if (n_gt == 0) return MPX_OK;
+  MPX_REQUIRE(h > 0 && w > 0 && 9ll * h * w < (1ll << 31), "mpx_bop_gt_info: bad image size %dx%d", h, w);
+  MPX_REQUIRE(n_img > 0, "mpx_bop_gt_info: n_img=%d", n_img);
+  MPX_DEVICE(d_depth_test);
+  MPX_DEVICE(d_depth_scale);
+  MPX_DEVICE(d_K);
+  MPX_DEVICE(d_depth_gt_large);
+  MPX_DEVICE(d_img_idx);
+  MPX_DEVICE(d_counts);
+  MPX_DEVICE(d_bbox);
+  MPX_DEVICE_OR_NULL(d_mask);
+  MPX_DEVICE_OR_NULL(d_mask_visib);
+  return bop_gt_info(n_gt, h, w, d_depth_test, n_img, d_depth_scale, d_K, d_depth_gt_large, d_img_idx, delta, d_counts,
+                     d_bbox, d_mask, d_mask_visib, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

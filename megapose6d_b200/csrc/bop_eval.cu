@@ -31,6 +31,19 @@ __device__ __forceinline__ double dist_from_depth(double X, double Y, double d) 
   return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(a, a), __dmul_rn(b, b)), __dmul_rn(d, d)));
 }
 
+// misc.depth_im_to_dist_im (calc_gt_masks.py): X d = ((x - cx) d) (1 / fx) in float64, then the same norm
+__device__ __forceinline__ double dist_from_depth_px(double xc, double yc, double rfx, double rfy, double d) {
+  const double a = __dmul_rn(__dmul_rn(xc, d), rfx);
+  const double b = __dmul_rn(__dmul_rn(yc, d), rfy);
+  return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(a, a), __dmul_rn(b, b)), __dmul_rn(d, d)));
+}
+
+// visibility.estimate_visib_mask_gt, "bop19" mode: fp32(dist_model) - fp32(dist_test) <= delta, or no test depth, and a
+// model surface
+__device__ __forceinline__ bool visib_bop19(double dist_model, float dist_test_f32, bool test_missing, float delta) {
+  return (__fsub_rn(__double2float_rn(dist_model), dist_test_f32) <= delta || test_missing) && dist_model > 0.0;
+}
+
 __device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -78,9 +91,8 @@ __global__ void __launch_bounds__(kVsdThreads) bop_vsd_count_kernel(
     const double dist_g = dist_from_depth(X, Y, static_cast<double>(dg));
     const float ft = __double2float_rn(dist_t);
     const bool test_missing = dist_t == 0.0;
-    const bool vg = (__fsub_rn(__double2float_rn(dist_g), ft) <= delta || test_missing) && dist_g > 0.0;
-    const bool ve = ((__fsub_rn(__double2float_rn(dist_e), ft) <= delta || test_missing) && dist_e > 0.0) ||
-                    (vg && dist_e > 0.0);
+    const bool vg = visib_bop19(dist_g, ft, test_missing, delta);
+    const bool ve = visib_bop19(dist_e, ft, test_missing, delta) || (vg && dist_e > 0.0);
     n_union += (vg || ve);
     if (vg && ve) {
       ++n_inter;
@@ -150,6 +162,157 @@ int bop_vsd(int n_pairs, int h, int w, const uint16_t* test, int n_img, const fl
   }
   bop_vsd_finish_kernel<<<(n_pairs + 127) / 128, 128, 0, stream>>>(n_pairs, n_taus, est_idx, gt_idx, img_idx, n_est, n_gt,
                                                                    n_img, cnt, err);
+  MPX_CHECK_CUDA(cudaGetLastError());
+  ++g_launches;
+  return MPX_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// ground-truth annotation (scripts/calc_gt_info.py, calc_gt_masks.py)
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int kGtThreads = 256;
+constexpr int kGtPixelsPerThread = 16;
+constexpr int kGtBoxWords = 8;  // {obj, visib} x {-xmin, -ymin, xmax, ymax} while counting: every slot is a running max
+constexpr int kGtBoxInit = static_cast<int>(0x80808080u);  // cudaMemset byte 0x80: below any coordinate
+
+__device__ __forceinline__ bool gt_img_valid(const int* img_idx, int g, int n_img) {
+  const int i = img_idx[g];
+  return i >= 0 && i < n_img;
+}
+
+// counts[g] = {px_count_all, px_count_valid, px_count_visib}, zeroed before the launch; box[g] as kGtBoxWords above.
+// One CTA row per gt (grid-stride over gts in y), grid-stride over the 3h x 3w canvas in x.
+__global__ void __launch_bounds__(kGtThreads) bop_gt_info_count_kernel(
+    int n_gt, int h, int w, const uint16_t* __restrict__ test, int n_img, const float* __restrict__ depth_scale,
+    const double* __restrict__ K, const float* __restrict__ large, const int* __restrict__ img_idx, float delta,
+    unsigned long long* __restrict__ counts, int* __restrict__ box, uint8_t* __restrict__ mask,
+    uint8_t* __restrict__ mask_visib) {
+  const int W = 3 * w, HW = 9 * h * w, hw = h * w;
+  __shared__ unsigned long long part_n[kGtThreads / 32][3];
+  __shared__ int part_b[kGtThreads / 32][kGtBoxWords];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int g = blockIdx.y; g < n_gt; g += gridDim.y) {
+    const bool ok = gt_img_valid(img_idx, g, n_img);
+    const int img = ok ? img_idx[g] : 0;
+    const uint16_t* t_im = test + static_cast<size_t>(img) * hw;
+    const float* l_im = large + static_cast<size_t>(g) * HW;
+    const double* k = K + 9 * img;
+    const double fx = k[0], cx = k[2], fy = k[4], cy = k[5];
+    const double rfx = __ddiv_rn(1.0, fx), rfy = __ddiv_rn(1.0, fy);
+    const float scale = depth_scale[img];
+    unsigned n_all = 0, n_valid = 0, n_visib = 0;
+    int b[kGtBoxWords];
+#pragma unroll
+    for (int j = 0; j < kGtBoxWords; ++j) b[j] = kGtBoxInit;
+
+    // the running index is 64-bit: its last step may pass INT_MAX for canvases near the 2^31-pixel limit
+    for (long long p = blockIdx.x * blockDim.x + threadIdx.x; p < HW; p += static_cast<long long>(gridDim.x) * blockDim.x) {
+      const int px = static_cast<int>(p);
+      const int Y = px / W, X = px - Y * W;
+      const int x = X - w, y = Y - h;  // image coordinates (the canvas' principal point is shifted by (w, h))
+      const bool in_image = x >= 0 && x < w && y >= 0 && y < h;
+      const float dl = ok ? l_im[px] : 0.f;
+      bool m = false, mv = false;
+      if (dl > 0.f) {
+        ++n_all;
+        b[0] = max(b[0], -x);
+        b[1] = max(b[1], -y);
+        b[2] = max(b[2], x);
+        b[3] = max(b[3], y);
+        if (in_image) {
+          const float dg = __fmul_rn(dl, 1000.f);
+          const float dt = __fmul_rn(static_cast<float>(t_im[y * w + x]), scale);
+          const double xc = __dadd_rn(static_cast<double>(x), -cx), yc = __dadd_rn(static_cast<double>(y), -cy);
+          // scene_gt_info: misc.depth_im_to_dist_im_fast, as the VSD kernel
+          const double Xf = __ddiv_rn(xc, fx), Yf = __ddiv_rn(yc, fy);
+          const double dist_t = dist_from_depth(Xf, Yf, static_cast<double>(dt));
+          const double dist_g = dist_from_depth(Xf, Yf, static_cast<double>(dg));
+          n_valid += dist_g > 0.0 && dist_t > 0.0;
+          if (visib_bop19(dist_g, __double2float_rn(dist_t), dist_t == 0.0, delta)) {
+            ++n_visib;
+            b[4] = max(b[4], -x);
+            b[5] = max(b[5], -y);
+            b[6] = max(b[6], x);
+            b[7] = max(b[7], y);
+          }
+          // mask / mask_visib: misc.depth_im_to_dist_im, whose rounding differs
+          const double dist_ts = dist_from_depth_px(xc, yc, rfx, rfy, static_cast<double>(dt));
+          const double dist_gs = dist_from_depth_px(xc, yc, rfx, rfy, static_cast<double>(dg));
+          m = dist_gs > 0.0;
+          mv = visib_bop19(dist_gs, __double2float_rn(dist_ts), dist_ts == 0.0, delta);
+        }
+      }
+      if (in_image) {
+        const size_t o = static_cast<size_t>(g) * hw + y * w + x;
+        if (mask) mask[o] = m;
+        if (mask_visib) mask_visib[o] = mv;
+      }
+    }
+
+    unsigned long long v0 = warp_sum_u64(n_all), v1 = warp_sum_u64(n_valid), v2 = warp_sum_u64(n_visib);
+#pragma unroll
+    for (int j = 0; j < kGtBoxWords; ++j) b[j] = __reduce_max_sync(0xffffffffu, b[j]);
+    if (lane == 0) {
+      part_n[warp][0] = v0;
+      part_n[warp][1] = v1;
+      part_n[warp][2] = v2;
+#pragma unroll
+      for (int j = 0; j < kGtBoxWords; ++j) part_b[warp][j] = b[j];
+    }
+    __syncthreads();
+    if (threadIdx.x < 3) {
+      unsigned long long s = 0;
+      for (int i = 0; i < kGtThreads / 32; ++i) s += part_n[i][threadIdx.x];
+      if (s) atomicAdd(counts + 3 * static_cast<size_t>(g) + threadIdx.x, s);
+    } else if (threadIdx.x >= 32 && threadIdx.x < 32 + kGtBoxWords) {
+      const int j = threadIdx.x - 32;
+      int s = kGtBoxInit;
+      for (int i = 0; i < kGtThreads / 32; ++i) s = max(s, part_b[i][j]);
+      if (s != kGtBoxInit) atomicMax(box + kGtBoxWords * static_cast<size_t>(g) + j, s);
+    }
+    __syncthreads();  // part_* are rewritten by the next gt
+  }
+}
+
+// box[g]: running maxima -> {bbox_obj, bbox_visib} as misc.calc_2d_bbox (x, y, x_max - x_min, y_max - y_min), both
+// [-1, -1, -1, -1] unless px_count_visib > 0; a gt with an out-of-range image index gets counts and boxes of -1
+__global__ void bop_gt_info_finish_kernel(int n_gt, int n_img, const int* __restrict__ img_idx,
+                                          unsigned long long* __restrict__ counts, int* __restrict__ box) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n_gt) return;
+  int* bx = box + kGtBoxWords * static_cast<size_t>(g);
+  unsigned long long* c = counts + 3 * static_cast<size_t>(g);
+  const bool ok = gt_img_valid(img_idx, g, n_img);
+  if (!ok) c[0] = c[1] = c[2] = ~0ull;
+  if (!ok || c[2] == 0) {
+    for (int j = 0; j < kGtBoxWords; ++j) bx[j] = -1;
+    return;
+  }
+  for (int k = 0; k < 2; ++k) {
+    int* q = bx + 4 * k;
+    const int x0 = -q[0], y0 = -q[1], x1 = q[2], y1 = q[3];
+    q[0] = x0;
+    q[1] = y0;
+    q[2] = x1 - x0;
+    q[3] = y1 - y0;
+  }
+}
+
+int bop_gt_info(int n_gt, int h, int w, const uint16_t* test, int n_img, const float* depth_scale, const double* K,
+                const float* large, const int* img_idx, float delta, int64_t* counts, int* bbox, uint8_t* mask,
+                uint8_t* mask_visib, cudaStream_t stream) {
+  if (n_gt == 0) return MPX_OK;
+  MPX_CHECK_CUDA(cudaMemsetAsync(counts, 0, sizeof(int64_t) * 3 * static_cast<size_t>(n_gt), stream));
+  MPX_CHECK_CUDA(cudaMemsetAsync(bbox, 0x80, sizeof(int) * kGtBoxWords * static_cast<size_t>(n_gt), stream));
+  const long long HW = 9ll * h * w;
+  const int bx = static_cast<int>((HW + kGtThreads * kGtPixelsPerThread - 1) / (kGtThreads * kGtPixelsPerThread));
+  const int by = n_gt < 65535 ? n_gt : 65535;  // gridDim.y limit: the kernel strides over the rest
+  auto* cnt = reinterpret_cast<unsigned long long*>(counts);
+  bop_gt_info_count_kernel<<<dim3(bx, by), kGtThreads, 0, stream>>>(n_gt, h, w, test, n_img, depth_scale, K, large,
+                                                                    img_idx, delta, cnt, bbox, mask, mask_visib);
+  MPX_CHECK_CUDA(cudaGetLastError());
+  ++g_launches;
+  bop_gt_info_finish_kernel<<<(n_gt + 127) / 128, 128, 0, stream>>>(n_gt, n_img, img_idx, cnt, bbox);
   MPX_CHECK_CUDA(cudaGetLastError());
   ++g_launches;
   return MPX_OK;

@@ -297,6 +297,9 @@ int bop_point_errors(int kind, int n_pairs, int n_models, const double* pts, con
                      const double* syms, const int64_t* sym_off, long long n_syms_total, const int* model_idx,
                      const double* pose_est, const double* pose_gt, const double* K, double* err, int* sym_argmin,
                      cudaStream_t stream);
+int bop_gt_info(int n_gt, int h, int w, const uint16_t* test, int n_img, const float* depth_scale, const double* K,
+                const float* large, const int* img_idx, float delta, int64_t* counts, int* bbox, uint8_t* mask,
+                uint8_t* mask_visib, cudaStream_t stream);
 
 
 // teaser.cu

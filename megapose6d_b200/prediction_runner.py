@@ -472,15 +472,26 @@ def run_predictions(scene_ds: SceneDataset, pose_estimator, inference_cfg: Infer
 def main(argv: Optional[List[str]] = None) -> None:
     """python -m megapose6d_b200.prediction_runner <frame_dir> [<frame_dir> ...] --model <name> --save-dir <dir>
     Frames in the README example's layout; the meshes are read from `--meshes-from` (default: the first frame directory).
+    python -m megapose6d_b200.prediction_runner --bop-dataset <dir> [--split test] [--label-format "{label}"] [--evaluate]
+    --model <name> --save-dir <dir>
+    The bop19 target frames of a BOP split (bop_dataset.keep_bop19(BOPDataset(...))) with the meshes of <dir>/models and the
+    ground truth as detections; `--evaluate` scores the 'refiner/final' CSV with bop_eval.BopEvaluator on rank 0, prints
+    the scores as one JSON line and saves them as <save-dir>/bop19_scores.json.
     Under torchrun the frames are sharded over the ranks (one process per GPU) and rank 0 writes the results."""
     import argparse
+    import json
     import os
 
     from .example import make_object_dataset
     from .load_model import NAMED_MODELS, load_named_model
 
-    parser = argparse.ArgumentParser(description="Pose predictions for a list of frames, BOP-format output")
-    parser.add_argument("frame_dirs", type=Path, nargs="+")
+    parser = argparse.ArgumentParser(description="Pose predictions for a list of frames or a BOP split, BOP-format output")
+    parser.add_argument("frame_dirs", type=Path, nargs="*")
+    parser.add_argument("--bop-dataset", type=Path, default=None, help="a dataset in the BOP format (instead of frame dirs)")
+    parser.add_argument("--split", default="test", help="split of --bop-dataset")
+    parser.add_argument("--label-format", default="{label}", help="object labels of --bop-dataset (the reference's "
+                        "label_format, e.g. 'ycbv-{label}')")
+    parser.add_argument("--evaluate", action="store_true", help="BOP 2019 scores of the predictions on --bop-dataset")
     parser.add_argument("--model", type=str, default="megapose-1.0-RGB-multi-hypothesis", choices=sorted(NAMED_MODELS))
     parser.add_argument("--models-root", type=Path, default=None)
     parser.add_argument("--meshes-from", type=Path, default=None)
@@ -488,6 +499,12 @@ def main(argv: Optional[List[str]] = None) -> None:
     parser.add_argument("--depth-refiner", choices=["icp", "teaserpp"], default=None,
                         help="refine the final poses against the frames' depth (evaluation/evaluation.py:132-139)")
     args = parser.parse_args(argv)
+    if bool(args.frame_dirs) == (args.bop_dataset is not None):
+        parser.error("give either frame directories or --bop-dataset")
+    if args.evaluate and args.bop_dataset is None:
+        parser.error("--evaluate needs --bop-dataset")
+    if args.bop_dataset is not None and args.meshes_from is not None:
+        parser.error("--meshes-from applies to frame directories; --bop-dataset reads <dir>/models")
     if "RANK" in os.environ and not dist.is_initialized():
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", 0)))
         dist.init_process_group("nccl")
@@ -498,7 +515,15 @@ def main(argv: Optional[List[str]] = None) -> None:
     cfg = InferenceConfig(detection_type="gt", n_refiner_iterations=params["n_refiner_iterations"],
                           n_pose_hypotheses=params["n_pose_hypotheses"], run_depth_refiner=args.depth_refiner is not None,
                           depth_refiner=args.depth_refiner, bsz_images=576, bsz_objects=16)
-    object_dataset = make_object_dataset(args.meshes_from or args.frame_dirs[0])
+    if args.bop_dataset is not None:
+        from .bop_dataset import BOPDataset, BOPObjectDataset, keep_bop19
+
+        object_dataset = BOPObjectDataset(args.bop_dataset / "models", label_format=args.label_format)
+        scene_ds = keep_bop19(BOPDataset(args.bop_dataset, label_format=args.label_format, split=args.split,
+                                         load_depth=info["requires_depth"]))
+    else:
+        object_dataset = make_object_dataset(args.meshes_from or args.frame_dirs[0])
+        scene_ds = ExampleDirSceneDataset(args.frame_dirs, load_depth=info["requires_depth"])
     pose_estimator = load_named_model(args.model, object_dataset, models_root=args.models_root).cuda()
     if args.depth_refiner is not None:
         from .icp_refiner import ICPRefiner
@@ -506,11 +531,17 @@ def main(argv: Optional[List[str]] = None) -> None:
 
         cls = ICPRefiner if args.depth_refiner == "icp" else TeaserppRefiner
         pose_estimator.depth_refiner = cls(pose_estimator.refiner_model.mesh_db, pose_estimator.refiner_model.renderer)
-    scene_ds = ExampleDirSceneDataset(args.frame_dirs, load_depth=info["requires_depth"])
     out = run_predictions(scene_ds, pose_estimator, cfg, save_dir=args.save_dir)
     if out["save_dir"] is not None:
         n = len(out["results"]["predictions"]["final"])
         print(f"wrote {n} pose(s) of {len(scene_ds)} frame(s) to {out['save_dir']}")
+        if args.evaluate:
+            from .bop_eval import BopEvaluator
+
+            csv = out["save_dir"] / "bop_refiner_final.csv"
+            scores = BopEvaluator(args.bop_dataset, args.split).evaluate(csv if csv.exists() else [])
+            (out["save_dir"] / "bop19_scores.json").write_text(json.dumps(scores))
+            print(json.dumps(scores))
     if dist.is_initialized():
         dist.destroy_process_group()
 
