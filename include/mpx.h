@@ -290,13 +290,51 @@ int mpx_net_create_preact(int c_pad, int out_dim, const int32_t* h_layer_blocks,
                           const float* const* h_conv_b, int n_convs, const float* const* h_block_affine, int n_blocks,
                           const float* d_head_w, const float* d_head_b, mpx_net** out);
 int mpx_net_destroy(mpx_net* net);
-/* mpx_net_forward replays a cached CUDA graph per (buffers, shape) after the first call; 0 disables that
- * (every launch is then issued eagerly on the caller's stream). Default: enabled. */
+/* mpx_net_forward and mpx_fpn_forward replay a cached CUDA graph per (buffers, shape) after the first call; 0 disables
+ * that (every launch is then issued eagerly on the caller's stream). Default: enabled. */
 int mpx_net_set_graphs(int on);
 size_t mpx_net_workspace_bytes(const mpx_net* net, int n, int h, int w);
 /* d_x: network input tensor (see above) for n samples of size h x w; d_out [n, out_dim] fp32 */
 int mpx_net_forward(const mpx_net* net, const void* d_x, int n, int h, int w, float* d_out,
                     void* d_workspace, size_t workspace_bytes, void* stream);
+
+/* ---- detector: ResNet-50 FPN + RPN head -----------------------------------------------------------
+ * The backbone (resnet_fpn_backbone("resnet50"): ResNet-50 v1.5 body with FrozenBatchNorm2d, returned layers 1-4,
+ * FeaturePyramidNetwork of 256 channels, LastLevelMaxPool) and the RPN head (RPNHead, conv_depth 1) of torchvision's
+ * Mask R-CNN (the reference's detector, models/mask_rcnn.py:23-46), for n images of one size.  Every convolution runs on
+ * the wgmma convolution (act16 operands and activations, fp32 accumulation, bias / residual / ReLU in the epilogue,
+ * one rounding per convolution); the FPN's top-down sum is the lateral convolution's residual.  63 convolutions, 71
+ * convolution launches, 78 launches in all.  megapose6d_b200/detector_engine.py builds the weights and drives it.
+ *
+ * mpx_fpn_create: h_conv_w / h_conv_b are HOST arrays of 63 DEVICE pointers in execution order, FrozenBatchNorm2d folded
+ * into the convolution before it (float64, the module's eps) and repacked as for mpx_net: act16 [C_out, R*S*C_in] with
+ * k = (r, s, c) and fp32 [C_out]:
+ *   0       stem, the 7x7/s2/p3 convolution as 4x4 over the space-to-depth input (c_pad 16)
+ *   1..52   per bottleneck of layer1..layer4 ([3, 4, 6, 3] blocks, widths 64/128/256/512, expansion 4, stride on the 3x3):
+ *           conv1 (1x1), conv2 (3x3), [downsample (1x1, stride s), block 0 only], conv3 (1x1)
+ *   53..56  FPN lateral 1x1 (inner_blocks 0..3, C_in 256/512/1024/2048 -> 256, with bias)
+ *   57..60  FPN output 3x3 (layer_blocks 0..3, 256 -> 256, with bias)
+ *   61      RPN 3x3 (256 -> 256), ReLU
+ *   62      RPN cls_logits and bbox_pred as one 1x1 256 -> 64: rows 0..A-1 objectness, A..5A-1 deltas, the rest zero
+ * n_anchors = A, 1..12.  The handle keeps the pointers; the tensors must outlive it. */
+typedef struct mpx_fpn mpx_fpn;
+int mpx_fpn_create(const void* const* h_conv_w, const float* const* h_conv_b, int n_convs, int n_anchors, mpx_fpn** out);
+int mpx_fpn_destroy(mpx_fpn* fpn);
+/* bytes of workspace for n images of h x w (0 for a size mpx_fpn_forward refuses) */
+size_t mpx_fpn_workspace_bytes(int n, int h, int w);
+/* d_images: fp32 NCHW [n, 3, h, w], the normalised, zero-padded batch of GeneralizedRCNNTransform (ImageList.tensors);
+ * h, w positive multiples of 32 (size_divisible = 32), so that every level is half the size of the one below.  Outputs
+ * are HOST arrays of 5 DEVICE pointers, one per level '0', '1', '2', '3', 'pool' (sizes h/4, h/8, h/16, h/32 and
+ * ceil(h/64) = P5[::2, ::2]; widths alike), caller-allocated fp32 NCHW:
+ *   h_features[l]   [n, 256, h_l, w_l]   the FPN outputs (the backbone's OrderedDict)
+ *   h_objectness[l] [n, A, h_l, w_l]     RPNHead's cls_logits
+ *   h_deltas[l]     [n, 4A, h_l, w_l]    RPNHead's bbox_pred
+ * Refused before any launch: a NULL handle, bad sizes, NULL or non-device pointers, a workspace smaller than
+ * mpx_fpn_workspace_bytes or not 256-byte aligned.  Replays a cached CUDA graph per (buffers, shape) from the second call
+ * on, like mpx_net_forward; mpx_net_set_graphs(0) turns that off for both. */
+int mpx_fpn_forward(const mpx_fpn* fpn, const float* d_images, int n, int h, int w, float* const* h_features,
+                    float* const* h_objectness, float* const* h_deltas, void* d_workspace, size_t workspace_bytes,
+                    void* stream);
 
 /* ---- BOP 2019 pose errors ------------------------------------------------------------------------
  * The pose-error functions of the BOP toolkit (bop_toolkit_lib/pose_error.py: vsd, mssd, mspd, add, adi), vendored by the

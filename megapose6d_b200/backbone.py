@@ -26,13 +26,15 @@ LAYERS = [3, 4, 6, 3]
 BN_EPS = 1e-5
 
 
-def _fold(sd: Dict[str, torch.Tensor], conv: str, bn: str) -> Tuple[torch.Tensor, torch.Tensor]:
+def _fold(sd: Dict[str, torch.Tensor], conv: str, bn: str, eps: float = BN_EPS) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Eval-mode BatchNorm (or torchvision's FrozenBatchNorm2d, same four tensors) `bn` folded into the bias-free
+    convolution `conv`, in float64; `eps` is the norm module's."""
     w = sd[conv + ".weight"].detach().double().cpu()
     g = sd[bn + ".weight"].detach().double().cpu()
     beta = sd[bn + ".bias"].detach().double().cpu()
     mean = sd[bn + ".running_mean"].detach().double().cpu()
     var = sd[bn + ".running_var"].detach().double().cpu()
-    scale = g / torch.sqrt(var + BN_EPS)
+    scale = g / torch.sqrt(var + eps)
     return w * scale.view(-1, 1, 1, 1), beta - mean * scale
 
 

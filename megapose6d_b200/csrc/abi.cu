@@ -653,4 +653,60 @@ int mpx_bop_gt_info(int n_gt, int h, int w, const uint16_t* d_depth_test, int n_
                      d_bbox, d_mask, d_mask_visib, static_cast<cudaStream_t>(stream));
 }
 
+// ---- detector: ResNet-50 FPN + RPN head ----
+struct mpx_fpn {
+  Fpn* fpn;
+};
+
+int mpx_fpn_create(const void* const* h_conv_w, const float* const* h_conv_b, int n_convs, int n_anchors, mpx_fpn** out) {
+  MPX_NOT_NULL(h_conv_w);
+  MPX_NOT_NULL(h_conv_b);
+  MPX_NOT_NULL(out);
+  MPX_REQUIRE(n_convs == kFpnConvs, "mpx_fpn_create: expected %d conv tensors, got %d", kFpnConvs, n_convs);
+  for (int i = 0; i < n_convs; ++i)
+    MPX_REQUIRE(is_device_ptr(h_conv_w[i]) && is_device_ptr(h_conv_b[i]),
+                "mpx_fpn_create: conv %d has a NULL or non-device tensor", i);
+  Fpn* fpn = nullptr;
+  int rc = fpn_create(h_conv_w, h_conv_b, n_convs, n_anchors, &fpn);
+  if (rc != MPX_OK) return rc;
+  *out = new mpx_fpn{fpn};
+  return MPX_OK;
+}
+
+int mpx_fpn_destroy(mpx_fpn* fpn) {
+  if (fpn) {
+    fpn_destroy(fpn->fpn);
+    delete fpn;
+  }
+  return MPX_OK;
+}
+
+static bool fpn_size_ok(int n, int h, int w) {
+  return n >= 1 && h >= 32 && w >= 32 && h % 32 == 0 && w % 32 == 0 &&
+         static_cast<long long>(n) * (h / 2) * (w / 2) < (1ll << 31);
+}
+
+size_t mpx_fpn_workspace_bytes(int n, int h, int w) { return fpn_size_ok(n, h, w) ? fpn_workspace_bytes(n, h, w) : 0; }
+
+int mpx_fpn_forward(const mpx_fpn* fpn, const float* d_images, int n, int h, int w, float* const* h_features,
+                    float* const* h_objectness, float* const* h_deltas, void* d_workspace, size_t workspace_bytes,
+                    void* stream) {
+  MPX_NOT_NULL(fpn);
+  MPX_REQUIRE(fpn_size_ok(n, h, w),
+              "mpx_fpn_forward: n=%d, %dx%d: need n >= 1, h and w positive multiples of 32, n*(h/2)*(w/2) < 2^31", n, h, w);
+  MPX_DEVICE(d_images);
+  MPX_NOT_NULL(h_features);
+  MPX_NOT_NULL(h_objectness);
+  MPX_NOT_NULL(h_deltas);
+  for (int l = 0; l < 5; ++l) {
+    MPX_REQUIRE(is_device_ptr(h_features[l]) && is_device_ptr(h_objectness[l]) && is_device_ptr(h_deltas[l]),
+                "mpx_fpn_forward: an output of level %d is NULL or not device memory", l);
+  }
+  MPX_DEVICE(d_workspace);
+  MPX_REQUIRE(workspace_bytes >= fpn_workspace_bytes(n, h, w), "mpx_fpn_forward: workspace of %zu bytes < %zu",
+              workspace_bytes, fpn_workspace_bytes(n, h, w));
+  return fpn_forward(fpn->fpn, d_images, n, h, w, h_features, h_objectness, h_deltas, d_workspace, workspace_bytes,
+                     static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

@@ -258,6 +258,8 @@ struct ConvCfg {
   static constexpr int kStages = (BLOCK_N == 256) ? 4 : (BLOCK_N == 128 ? 6 : 8);  // 192 KiB of stages
   static constexpr int kSmemBytes =
       kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + 2048 /*bias, C_out <= 512*/;
+  // launches with C_out > 512 (the detector's layer3 / layer4, up to 2048) stage C_out * 4 B of bias instead
+  static int smem_bytes(int c_out) { return c_out <= 512 ? kSmemBytes : kSmemBytes - 2048 + 4 * c_out; }
   // split-K: fp32 partial tile parked in the drained stages; +16 B per row keeps the row-owner stores conflict-free
   static constexpr int kParkPitch = BLOCK_N * 4 + 16;
   static_assert(kBlockM * kParkPitch <= kStages * kStageBytes, "split-K tile does not fit the pipeline stages");
@@ -976,18 +978,18 @@ template <int BLOCK_N>
 static int launch_conv(const CUtensorMap& ma, const CUtensorMap& mb, const ConvParams& p, cudaStream_t stream,
                        int max_ctas) {
   using Cfg = ConvCfg<BLOCK_N>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    MPX_CHECK_CUDA(cudaFuncSetAttribute(conv_wgmma_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        Cfg::kSmemBytes));
-    attr_set = true;
+  const int smem = Cfg::smem_bytes(p.C_out);
+  static int attr_bytes = 0;  // the largest dynamic shared-memory size set on this instantiation so far
+  if (smem > attr_bytes) {
+    MPX_CHECK_CUDA(cudaFuncSetAttribute(conv_wgmma_kernel<BLOCK_N>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr_bytes = smem;
   }
   int grid = p.m_tiles * p.n_tiles * p.splits;
   const int cap = max_ctas > 0 ? max_ctas : sm_count();
   ProfileSlot* slot = profile_begin(stream);
   // split-K: one work item per CTA, the k-splits of a tile form a cluster
   if (p.splits == 1 && grid > cap) grid = cap;
-  MPX_CHECK_CUDA(launch_pdl(conv_wgmma_kernel<BLOCK_N>, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, stream, p.splits,
+  MPX_CHECK_CUDA(launch_pdl(conv_wgmma_kernel<BLOCK_N>, dim3(grid), dim3(kThreads), smem, stream, p.splits,
                             ma, mb, p));
   MPX_CHECK_CUDA(cudaGetLastError());
   ++g_launches;
@@ -1183,9 +1185,11 @@ static int conv64_forward(const ConvDesc& d, const void* x, const void* w, const
 // residual/out: [n_img, P, Q, C_out] act16.
 int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* bias,
                  const void* residual, void* out, int block_n_override, int max_ctas,
-                 cudaStream_t stream, int splitk) {
+                 cudaStream_t stream, int splitk, int max_c_out) {
   MPX_REQUIRE(d.C_in % 64 == 0 && d.C_in >= 64, "conv: C_in=%d must be a multiple of 64", d.C_in);
-  MPX_REQUIRE(d.C_out % 64 == 0 && d.C_out <= 512, "conv: C_out=%d must be a multiple of 64, at most 512", d.C_out);
+  MPX_REQUIRE(max_c_out <= 2048, "conv: C_out limit %d above 2048", max_c_out);
+  MPX_REQUIRE(d.C_out % 64 == 0 && d.C_out <= max_c_out, "conv: C_out=%d must be a multiple of 64, at most %d", d.C_out,
+              max_c_out);
   MPX_REQUIRE(d.stride == 1 || d.stride == 2, "conv: stride %d unsupported", d.stride);
   MPX_REQUIRE(d.R >= 1 && d.R <= 8 && d.S >= 1 && d.S <= 8, "conv: filter %dx%d unsupported", d.R, d.S);
   // the pooled epilogue needs non-negative values (ReLU) and no residual; refused without an error text otherwise

@@ -184,9 +184,11 @@ struct ConvDesc {
                  //    when no kernel with that epilogue serves the shape
 };
 // splitk: 0 = never, -1 = heuristic (few output tiles, long K loop), 1|2|4|8 = that many k-splits (cluster size)
+// max_c_out: the largest C_out the caller accepts (512 for the single-convolution entry points and the pose networks,
+// 2048 for the detector plan); C_out > 512 stages 4 * C_out bytes of bias in shared memory
 int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* bias,
                  const void* residual, void* out, int block_n_override, int max_ctas,
-                 cudaStream_t stream, int splitk = 0);
+                 cudaStream_t stream, int splitk = 0, int max_c_out = 512);
 int conv_out_dim(int in, int pad_lo, int pad_hi, int k, int stride);
 int maxpool3x3s2(const void* x, int n, int h, int w, int c, void* out, cudaStream_t stream);
 int avgpool_linear(const void* x, int n, int hw, int c, const float* w, const float* b, int out_dim,
@@ -201,6 +203,16 @@ size_t net_workspace_bytes(const Net* net, int n, int h, int w);
 int net_forward(const Net* net, const void* x, int n, int h, int w, float* out, void* workspace,
                 size_t workspace_bytes, cudaStream_t stream);
 void net_destroy(Net* net);
+bool net_graphs_enabled();
+
+// detector_net.cu
+struct Fpn;
+constexpr int kFpnConvs = 63;  // stem, 16 bottlenecks x 3 + 4 downsamples, 4 lateral + 4 output FPN, RPN 3x3 + merged 1x1
+int fpn_create(const void* const* conv_w, const float* const* conv_b, int n_convs, int n_anchors, Fpn** out);
+void fpn_destroy(Fpn* fpn);
+size_t fpn_workspace_bytes(int n, int h, int w);
+int fpn_forward(Fpn* fpn, const float* images, int n, int h, int w, float* const* features, float* const* objectness,
+                float* const* deltas, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 // raster.cu
 struct MeshDb {

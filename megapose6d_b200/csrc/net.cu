@@ -220,6 +220,7 @@ struct Net {
 
 static bool g_use_graphs = true;
 void net_set_graphs(int on) { g_use_graphs = on != 0; }
+bool net_graphs_enabled() { return g_use_graphs; }
 
 static const int kLayerBlocks[4] = {3, 4, 6, 3};
 static const int kLayerWidth[4] = {64, 128, 256, 512};

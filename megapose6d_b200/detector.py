@@ -115,8 +115,11 @@ def create_model_detector(cfg, n_classes: int) -> torch.nn.Module:
                     max_size=max(cfg.input_resize), min_size=min(cfg.input_resize))
 
 
-def load_detector(run_id: str, models_root: Optional[Path] = None, device: str = "cuda") -> Detector:
-    """inference/utils.py:57-70: `<models_root>/<run_id>/{config.yaml, checkpoint.pth.tar}` -> Detector."""
+def load_detector(run_id: str, models_root: Optional[Path] = None, device: str = "cuda", engine: bool = False) -> Detector:
+    """inference/utils.py:57-70: `<models_root>/<run_id>/{config.yaml, checkpoint.pth.tar}` -> Detector.  `engine=True`
+    runs the Mask R-CNN's ResNet-50 FPN backbone and RPN head on the engine's wgmma convolutions
+    (`detector_engine.engine_model`; the rest of the model stays torchvision's); the default is torchvision's model
+    throughout, as in the reference."""
     from . import load_model
 
     run_dir = Path(models_root if models_root is not None else load_model.LOCAL_DATA_DIR / "experiments") / run_id  # EXP_DIR
@@ -127,4 +130,8 @@ def load_detector(run_id: str, models_root: Optional[Path] = None, device: str =
     model = model.to(device).eval()
     model.cfg = cfg
     model.config = cfg
+    if engine:
+        from .detector_engine import engine_model
+
+        model = engine_model(model, device)
     return Detector(model)

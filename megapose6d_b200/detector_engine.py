@@ -1,0 +1,273 @@
+"""The Mask R-CNN detector's ResNet-50 FPN backbone and RPN head on the engine's wgmma convolutions.
+
+`engine_model(model)` takes a torchvision `MaskRCNN` (what `detector.create_model_detector` builds, the reference's
+models/mask_rcnn.py:23-46) and returns a module that is called like it (`module(list_of_images)` in eval mode) and returns
+the same kind of detections.  The backbone (body + FPN) and `rpn.head` run as one `mpx_fpn_forward` (include/mpx.h,
+csrc/detector_net.cu); everything else is the model's own torchvision objects, run unchanged: the transform, the anchor
+generator, proposal decoding and filtering, the RoI heads and the postprocessing.  The model itself is not modified.
+
+Weights are repacked once:
+  * FrozenBatchNorm2d folded into the convolution before it, in float64 with the module's eps (`backbone._fold`);
+  * the 7x7/s2 stem rewritten as the 4x4 convolution over the space-to-depth input (`backbone._stem_s2d`, c_pad 16);
+  * `cls_logits` (A rows) and `bbox_pred` (4A rows) merged into one 1x1 convolution of 64 rows, the rest zero;
+  * every matrix rounded once to the library's 16-bit type, saturating.
+"""
+from __future__ import annotations
+
+import ctypes
+from collections import OrderedDict
+from typing import Dict, List, NamedTuple, Optional, Tuple
+
+import torch
+from torch import nn
+
+from . import _abi
+from .backbone import _fold, _pack, _stem_s2d
+
+C_PAD = 16  # space-to-depth channels per sub-pixel: 3 colour channels, zero-padded
+LAYERS = [3, 4, 6, 3]
+WIDTHS = [64, 128, 256, 512]
+FPN_IN = [256, 512, 1024, 2048]
+FPN_CHANNELS = 256
+HEAD_ROWS = 64  # merged RPN 1x1: A objectness rows + 4A delta rows, zero-padded
+MAX_ANCHORS = HEAD_ROWS // 5
+LEVELS = ["0", "1", "2", "3", "pool"]
+
+
+class PlanConv(NamedTuple):
+    """One convolution of the plan, as the engine runs it (stem: as the torchvision 7x7 module it replaces)."""
+    modules: Tuple[str, ...]  # Conv2d module name(s); two for the merged RPN 1x1
+    norm: Optional[str]       # FrozenBatchNorm2d folded into it, or None (the convolution has its own bias)
+    kernel: int
+    stride: int
+    padding: int
+    c_in: int
+    c_out: int
+
+
+def weight_plan(n_anchors: int) -> List[PlanConv]:
+    """The 63 convolutions in the order mpx_fpn_create takes them (include/mpx.h)."""
+    body = "backbone.body"
+    plan = [PlanConv((f"{body}.conv1",), f"{body}.bn1", 7, 2, 3, 3, 64)]
+    c_in = 64
+    for li, (nb, width) in enumerate(zip(LAYERS, WIDTHS)):
+        for bi in range(nb):
+            p = f"{body}.layer{li + 1}.{bi}"
+            stride = 2 if bi == 0 and li > 0 else 1
+            plan.append(PlanConv((p + ".conv1",), p + ".bn1", 1, 1, 0, c_in, width))
+            plan.append(PlanConv((p + ".conv2",), p + ".bn2", 3, stride, 1, width, width))
+            if bi == 0:
+                plan.append(PlanConv((p + ".downsample.0",), p + ".downsample.1", 1, stride, 0, c_in, 4 * width))
+            plan.append(PlanConv((p + ".conv3",), p + ".bn3", 1, 1, 0, width, 4 * width))
+            c_in = 4 * width
+    for i, c in enumerate(FPN_IN):
+        plan.append(PlanConv((f"backbone.fpn.inner_blocks.{i}.0",), None, 1, 1, 0, c, FPN_CHANNELS))
+    for i in range(4):
+        plan.append(PlanConv((f"backbone.fpn.layer_blocks.{i}.0",), None, 3, 1, 1, FPN_CHANNELS, FPN_CHANNELS))
+    plan.append(PlanConv(("rpn.head.conv.0.0",), None, 3, 1, 1, FPN_CHANNELS, FPN_CHANNELS))
+    plan.append(PlanConv(("rpn.head.cls_logits", "rpn.head.bbox_pred"), None, 1, 1, 0, FPN_CHANNELS, 5 * n_anchors))
+    return plan
+
+
+def _refuse(what: str) -> None:
+    raise NotImplementedError(f"engine_model: {what} is not served by the engine's ResNet-50 FPN plan")
+
+
+def check_supported(model: nn.Module) -> int:
+    """Raises NotImplementedError for a structure the plan does not serve; returns the anchors per location."""
+    from torchvision.models.detection.backbone_utils import BackboneWithFPN
+    from torchvision.models.detection.generalized_rcnn import GeneralizedRCNN
+    from torchvision.models.resnet import Bottleneck
+    from torchvision.ops.feature_pyramid_network import LastLevelMaxPool
+    from torchvision.ops.misc import FrozenBatchNorm2d
+
+    if not isinstance(model, GeneralizedRCNN) or not hasattr(model, "rpn"):
+        _refuse(f"a {type(model).__name__}")
+    if getattr(model.transform, "size_divisible", None) != 32:
+        _refuse(f"size_divisible={getattr(model.transform, 'size_divisible', None)}")
+    bb = model.backbone
+    if not isinstance(bb, BackboneWithFPN):
+        _refuse(f"the backbone {type(bb).__name__}")
+    body = bb.body
+    if dict(body.return_layers) != {"layer1": "0", "layer2": "1", "layer3": "2", "layer4": "3"}:
+        _refuse(f"returned layers {dict(body.return_layers)}")
+    for li, nb in enumerate(LAYERS):
+        layer = getattr(body, f"layer{li + 1}", None)
+        if layer is None or len(layer) != nb or not all(isinstance(b, Bottleneck) for b in layer):
+            _refuse(f"layer{li + 1} (the ResNet-50 body has [3, 4, 6, 3] Bottleneck blocks)")
+    if not isinstance(bb.fpn.extra_blocks, LastLevelMaxPool):
+        _refuse(f"the FPN extra block {type(bb.fpn.extra_blocks).__name__}")
+    if bb.out_channels != FPN_CHANNELS:
+        _refuse(f"an FPN of {bb.out_channels} channels")
+    for blocks in (bb.fpn.inner_blocks, bb.fpn.layer_blocks):
+        if len(blocks) != 4 or any(len(b) != 1 for b in blocks):
+            _refuse("an FPN with a norm layer or other than four levels")
+    head = model.rpn.head
+    if len(head.conv) != 1:
+        _refuse(f"an RPN head with conv_depth={len(head.conv)}")
+    n_anchors = head.cls_logits.out_channels
+    if n_anchors > MAX_ANCHORS or head.bbox_pred.out_channels != 4 * n_anchors:
+        _refuse(f"{n_anchors} anchors per location (at most {MAX_ANCHORS})")
+    mods = dict(model.named_modules())
+    for pc in weight_plan(n_anchors):
+        if pc.norm is not None and type(mods.get(pc.norm)) is not FrozenBatchNorm2d:
+            _refuse(f"the norm {type(mods.get(pc.norm)).__name__} at {pc.norm} (FrozenBatchNorm2d only)")
+        for name in pc.modules:
+            conv = mods.get(name)
+            if not isinstance(conv, nn.Conv2d):
+                _refuse(f"{name} (not a Conv2d)")
+            if conv.dilation != (1, 1) or conv.groups != 1:
+                _refuse(f"dilation {conv.dilation} / groups {conv.groups} at {name}")
+            k = pc.kernel
+            if (conv.kernel_size != (k, k) or conv.stride != (pc.stride, pc.stride) or conv.padding != (pc.padding,) * 2
+                    or conv.in_channels != pc.c_in or (len(pc.modules) == 1 and conv.out_channels != pc.c_out)
+                    or (conv.bias is None) != (pc.norm is not None)):
+                _refuse(f"the convolution {name} {tuple(conv.weight.shape)} stride {conv.stride} padding {conv.padding}")
+    mp = body.maxpool
+    if (mp.kernel_size, mp.stride, mp.padding) != (3, 2, 1):
+        _refuse("the stem max-pool")
+    return n_anchors
+
+
+def fold_plan(model: nn.Module, n_anchors: int) -> List[Tuple[torch.Tensor, torch.Tensor]]:
+    """float64 (weight OIHW, bias) per plan entry: norms folded, the RPN 1x1 merged and zero-padded to 64 rows."""
+    sd = model.state_dict()
+    mods = dict(model.named_modules())
+    out = []
+    for pc in weight_plan(n_anchors):
+        if pc.norm is not None:
+            out.append(_fold(sd, pc.modules[0], pc.norm, eps=mods[pc.norm].eps))
+            continue
+        w = torch.cat([sd[m + ".weight"].detach().double().cpu() for m in pc.modules])
+        b = torch.cat([sd[m + ".bias"].detach().double().cpu() for m in pc.modules])
+        if len(pc.modules) > 1:
+            w = torch.cat([w, w.new_zeros(HEAD_ROWS - w.shape[0], *w.shape[1:])])
+            b = torch.cat([b, b.new_zeros(HEAD_ROWS - b.shape[0])])
+        out.append((w, b))
+    return out
+
+
+def to_act16(t: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """float -> the 16-bit type, round-to-nearest-even through fp32, saturating at the type's largest finite value."""
+    lim = float(torch.finfo(dtype).max)
+    return t.to(torch.float32).clamp(-lim, lim).to(dtype)
+
+
+def level_sizes(h: int, w: int) -> List[Tuple[int, int]]:
+    """(h_l, w_l) of the levels '0', '1', '2', '3', 'pool' for a padded batch of h x w (multiples of 32)."""
+    sizes = [(h >> l, w >> l) for l in range(2, 6)]
+    return sizes + [((sizes[-1][0] + 1) // 2, (sizes[-1][1] + 1) // 2)]
+
+
+class FpnEngine:
+    """Owns the repacked device weights and the mpx_fpn handle.  `run(images)` returns the FPN features, objectness and
+    deltas of a padded fp32 batch [n, 3, h, w] as lists of five fp32 NCHW tensors.  The tensors are the engine's own
+    output buffers, one set per shape, overwritten by the next call of that shape."""
+
+    def __init__(self, model: nn.Module, device="cuda"):
+        self.n_anchors = check_supported(model)
+        self.device = torch.device(device)
+        act = _abi.act_dtype()
+        self._weights: List[torch.Tensor] = []
+        self._biases: List[torch.Tensor] = []
+        for i, (w, b) in enumerate(fold_plan(model, self.n_anchors)):
+            wmat = _stem_s2d(w, C_PAD) if i == 0 else _pack(w)
+            self._weights.append(to_act16(wmat, act).to(self.device).contiguous())
+            self._biases.append(b.to(torch.float32).to(self.device).contiguous())
+        n = len(self._weights)
+        wp = (ctypes.c_void_p * n)(*[t.data_ptr() for t in self._weights])
+        bp = (ctypes.c_void_p * n)(*[t.data_ptr() for t in self._biases])
+        handle = ctypes.c_void_p()
+        _abi.check(_abi.lib().mpx_fpn_create(wp, bp, n, self.n_anchors, ctypes.byref(handle)))
+        self._handle = handle
+        self._workspace: Optional[torch.Tensor] = None
+        self._outputs: Dict[Tuple[int, int, int], Tuple[List[torch.Tensor], ...]] = {}
+
+    def __del__(self):
+        try:
+            if getattr(self, "_handle", None) is not None:
+                _abi.lib().mpx_fpn_destroy(self._handle)
+        except Exception:  # noqa: BLE001
+            pass
+
+    def run(self, images: torch.Tensor) -> Tuple[List[torch.Tensor], List[torch.Tensor], List[torch.Tensor]]:
+        n, c, h, w = images.shape
+        if c != 3 or images.dtype != torch.float32:
+            raise ValueError(f"FpnEngine.run: expected fp32 [n, 3, h, w], got {images.dtype} {tuple(images.shape)}")
+        images = images.contiguous()
+        need = _abi.lib().mpx_fpn_workspace_bytes(n, h, w)
+        if need and (self._workspace is None or self._workspace.numel() < need):
+            self._workspace = None
+            self._workspace = torch.empty(need, dtype=torch.uint8, device=self.device)
+        outs = self._outputs.get((n, h, w))
+        if outs is None:
+            sizes = level_sizes(h, w)
+            A = self.n_anchors
+
+            def alloc(ch):
+                return [torch.empty(n, ch, hl, wl, device=self.device) for hl, wl in sizes]
+
+            outs = self._outputs[(n, h, w)] = (alloc(FPN_CHANNELS), alloc(A), alloc(4 * A))
+        arrays = [(ctypes.c_void_p * 5)(*[t.data_ptr() for t in ts]) for ts in outs]
+        ws = self._workspace
+        _abi.check(_abi.lib().mpx_fpn_forward(self._handle, _abi.ptr(images), n, h, w, *arrays,
+                                              None if ws is None else ws.data_ptr(), 0 if ws is None else ws.numel(),
+                                              _abi.stream_ptr()))
+        return outs
+
+
+class EngineMaskRCNN(nn.Module):
+    """Called like torchvision's GeneralizedRCNN in eval mode: `module(images)` -> list of dicts(boxes, labels, scores,
+    masks).  Holds the model's transform, RPN and RoI heads by reference (not as submodules: it does not own them)."""
+
+    def __init__(self, model: nn.Module, device="cuda"):
+        super().__init__()
+        self.engine = FpnEngine(model, device)
+        self._stages = (model.transform, model.rpn, model.roi_heads)
+        for attr in ("config", "cfg"):
+            if hasattr(model, attr):
+                setattr(self, attr, getattr(model, attr))
+        self.train(False)
+
+    def train(self, mode: bool = True):
+        if mode:
+            raise NotImplementedError("the engine detector runs inference only")
+        return super().train(False)
+
+    def heads(self, image_list) -> Tuple["OrderedDict[str, torch.Tensor]", List[torch.Tensor], List[torch.Tensor]]:
+        """The backbone's feature OrderedDict and the RPN head's objectness / deltas of a transformed ImageList."""
+        feats, objectness, deltas = self.engine.run(image_list.tensors)
+        return OrderedDict(zip(LEVELS, feats)), objectness, deltas
+
+    def proposals(self, image_list, features, objectness, deltas) -> List[torch.Tensor]:
+        """RegionProposalNetwork.forward (eval) from the head's outputs: the model's anchor generator, box coder and
+        proposal filter."""
+        from torchvision.models.detection.rpn import concat_box_prediction_layers
+
+        rpn = self._stages[1]
+        anchors = rpn.anchor_generator(image_list, list(features.values()))
+        num_anchors_per_level = [o[0].numel() for o in objectness]
+        objectness, pred_bbox_deltas = concat_box_prediction_layers(objectness, deltas)
+        proposals = rpn.box_coder.decode(pred_bbox_deltas.detach(), anchors).view(len(anchors), -1, 4)
+        boxes, _ = rpn.filter_proposals(proposals, objectness, image_list.image_sizes, num_anchors_per_level)
+        return boxes
+
+    @torch.no_grad()
+    def forward(self, images: List[torch.Tensor], targets=None):
+        if targets is not None:
+            raise NotImplementedError("the engine detector runs inference only")
+        transform, _, roi_heads = self._stages
+        original_image_sizes = [(int(img.shape[-2]), int(img.shape[-1])) for img in images]
+        image_list, _ = transform(images)
+        features, objectness, deltas = self.heads(image_list)
+        proposals = self.proposals(image_list, features, objectness, deltas)
+        detections, _ = roi_heads(features, proposals, image_list.image_sizes)
+        return transform.postprocess(detections, image_list.image_sizes, original_image_sizes)
+
+
+def engine_model(model: nn.Module, device="cuda") -> EngineMaskRCNN:
+    """`model` (a torchvision MaskRCNN on `device`, in eval mode) with its backbone and RPN head on the engine.  Raises
+    NotImplementedError, before any device work, for a structure the plan does not serve: a backbone other than the
+    ResNet-50 body with FPN (returned layers 1-4, 256 channels, LastLevelMaxPool), a norm other than FrozenBatchNorm2d,
+    dilation, an RPN head with conv_depth != 1 or more than 12 anchors per location, size_divisible != 32."""
+    return EngineMaskRCNN(model, device)

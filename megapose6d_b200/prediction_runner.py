@@ -498,7 +498,14 @@ def main(argv: Optional[List[str]] = None) -> None:
     parser.add_argument("--save-dir", type=Path, required=True)
     parser.add_argument("--depth-refiner", choices=["icp", "teaserpp"], default=None,
                         help="refine the final poses against the frames' depth (evaluation/evaluation.py:132-139)")
+    parser.add_argument("--detector", type=str, default=None, metavar="RUN_ID",
+                        help="detect objects with this Mask R-CNN run (under --models-root) instead of using the ground "
+                        "truth as detections (detection_type='detector')")
+    parser.add_argument("--detector-engine", action="store_true",
+                        help="run the detector's ResNet-50 FPN backbone and RPN head on the engine's convolutions")
     args = parser.parse_args(argv)
+    if args.detector_engine and args.detector is None:
+        parser.error("--detector-engine needs --detector")
     if bool(args.frame_dirs) == (args.bop_dataset is not None):
         parser.error("give either frame directories or --bop-dataset")
     if args.evaluate and args.bop_dataset is None:
@@ -512,7 +519,7 @@ def main(argv: Optional[List[str]] = None) -> None:
     if args.depth_refiner is not None and not info["requires_depth"]:
         parser.error(f"--depth-refiner needs a model that loads depth; {args.model} does not")
     params = info["inference_parameters"]
-    cfg = InferenceConfig(detection_type="gt", n_refiner_iterations=params["n_refiner_iterations"],
+    cfg = InferenceConfig(detection_type="gt" if args.detector is None else "detector", n_refiner_iterations=params["n_refiner_iterations"],
                           n_pose_hypotheses=params["n_pose_hypotheses"], run_depth_refiner=args.depth_refiner is not None,
                           depth_refiner=args.depth_refiner, bsz_images=576, bsz_objects=16)
     if args.bop_dataset is not None:
@@ -531,6 +538,11 @@ def main(argv: Optional[List[str]] = None) -> None:
 
         cls = ICPRefiner if args.depth_refiner == "icp" else TeaserppRefiner
         pose_estimator.depth_refiner = cls(pose_estimator.refiner_model.mesh_db, pose_estimator.refiner_model.renderer)
+    if args.detector is not None:
+        from .detector import load_detector
+
+        pose_estimator.detector_model = load_detector(args.detector, models_root=args.models_root,
+                                                      engine=args.detector_engine)
     out = run_predictions(scene_ds, pose_estimator, cfg, save_dir=args.save_dir)
     if out["save_dir"] is not None:
         n = len(out["results"]["predictions"]["final"])
