@@ -48,7 +48,10 @@ __device__ __forceinline__ AxisTap axis_tap(float v, int size) {
 // depth-validity mask (only accumulated when WITH_DEPTH).  The per-axis work (bounds, floor, weights) is done
 // once per sample row / column instead of once per sample, and the 2x2 texel block of the previous sample is kept
 // in registers: with bins smaller than a pixel most of the 16 samples share it.  Every floating-point operation
-// and its order are those of torchvision's kernel.
+// and its order are those of torchvision's kernel, except that a tap of zero weight (a sample on an integer row /
+// column, or clamped to the last one) adds 0 instead of 0 * texel: a NaN or inf texel reached only through zero weights
+// does not make the sum NaN.  The collapsed form skips such taps, and a crop must not depend on which form its size
+// selects.  Finite texels give the same sums either way.
 template <bool WITH_DEPTH>
 __device__ __forceinline__ void roi_align_pixel(const float4* __restrict__ img, int h, int w, const RoiParams& r,
                                                 int ph, int pw, float4& acc, float& vacc) {
@@ -74,13 +77,17 @@ __device__ __forceinline__ void roi_align_pixel(const float4* __restrict__ img, 
         cy0 = ty.lo; cy1 = ty.hi; cx0 = tx[ix].lo; cx1 = tx[ix].hi;
       }
       const float w1 = ty.h * tx[ix].h, w2 = ty.h * tx[ix].l, w3 = ty.l * tx[ix].h, w4 = ty.l * tx[ix].l;
-      acc.x += w1 * v1.x + w2 * v2.x + w3 * v3.x + w4 * v4.x;
-      acc.y += w1 * v1.y + w2 * v2.y + w3 * v3.y + w4 * v4.y;
-      acc.z += w1 * v1.z + w2 * v2.z + w3 * v3.z + w4 * v4.z;
+      // the high taps weigh 0 exactly when l == 0 on their axis (h = 1 - l is never 0): their texels count as 0
+      const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+      const bool x0 = tx[ix].l == 0.f, y0 = ty.l == 0.f;
+      const float4 u2 = x0 ? z4 : v2, u3 = y0 ? z4 : v3, u4 = (x0 || y0) ? z4 : v4;
+      acc.x += w1 * v1.x + w2 * u2.x + w3 * u3.x + w4 * u4.x;
+      acc.y += w1 * v1.y + w2 * u2.y + w3 * u3.y + w4 * u4.y;
+      acc.z += w1 * v1.z + w2 * u2.z + w3 * u3.z + w4 * u4.z;
       if (WITH_DEPTH) {
-        acc.w += w1 * v1.w + w2 * v2.w + w3 * v3.w + w4 * v4.w;
-        vacc += w1 * (v1.w > 0.f ? 1.f : 0.f) + w2 * (v2.w > 0.f ? 1.f : 0.f) + w3 * (v3.w > 0.f ? 1.f : 0.f) +
-                w4 * (v4.w > 0.f ? 1.f : 0.f);
+        acc.w += w1 * v1.w + w2 * u2.w + w3 * u3.w + w4 * u4.w;
+        vacc += w1 * (v1.w > 0.f ? 1.f : 0.f) + w2 * (u2.w > 0.f ? 1.f : 0.f) + w3 * (u3.w > 0.f ? 1.f : 0.f) +
+                w4 * (u4.w > 0.f ? 1.f : 0.f);
       }
     }
   }
