@@ -336,6 +336,25 @@ int mpx_fpn_forward(const mpx_fpn* fpn, const float* d_images, int n, int h, int
                     float* const* h_objectness, float* const* h_deltas, void* d_workspace, size_t workspace_bytes,
                     void* stream);
 
+/* ---- detector: mask inference and pasting --------------------------------------------------------
+ * torchvision's maskrcnn_inference (sigmoid of the logits, the channel of each detection's label) followed by what
+ * GeneralizedRCNNTransform.postprocess does to boxes and masks: resize_boxes to the original image size and
+ * paste_masks_in_image (padding 1: the m x m probabilities zero-padded to m + 2, the box expanded about its centre by
+ * (m + 2) / m and truncated to integers, the map resized bilinearly (align_corners=False) to the box and pasted, clipped, into
+ * a zeroed image), for the detections of n_images images in one launch, with no host synchronisation.
+ *   d_logits [n_masks, n_classes, m, m] fp32   the mask predictor's logits, the detections of image 0 first
+ *   d_labels [n_masks] int64                   labels; a label outside 0..n_classes-1 gives an all-zero mask
+ *   d_boxes [n_masks, 4] fp32                  (x0, y0, x1, y1) in the transformed image's coordinates
+ *   h_counts [n_images]                        HOST: detections per image, adding up to n_masks
+ *   h_sizes [n_images, 4]                      HOST: (h, w) of the transformed image, (H, W) of the original image
+ * Outputs: d_boxes_out [n_masks, 4] fp32, the boxes resized to the original images; h_masks: HOST array of n_images DEVICE
+ * pointers, h_masks[i] [h_counts[i], 1, H_i, W_i] fp32 (may be NULL where h_counts[i] == 0).  The box arithmetic rounds as
+ * torchvision's fp32 operations do; the probabilities follow ATen's sigmoid and upsample_bilinear2d expressions.
+ * n_images 1..64, m 1..64, n_masks 0..65535.  Refused before any launch: bad sizes or counts, NULL or non-device pointers. */
+int mpx_mask_paste(const float* d_logits, const int64_t* d_labels, const float* d_boxes, int n_masks, int n_classes,
+                   int m, int n_images, const int32_t* h_counts, const int32_t* h_sizes, float* d_boxes_out,
+                   float* const* h_masks, void* stream);
+
 /* ---- BOP 2019 pose errors ------------------------------------------------------------------------
  * The pose-error functions of the BOP toolkit (bop_toolkit_lib/pose_error.py: vsd, mssd, mspd, add, adi), vendored by the
  * reference under deps/bop_toolkit_challenge; megapose6d_b200/bop_eval.py drives them.  Lengths are millimetres.

@@ -73,6 +73,8 @@ def _declare(lib: ctypes.CDLL) -> None:
     lib.mpx_fpn_workspace_bytes.argtypes = [c_int, c_int, c_int]
     lib.mpx_fpn_workspace_bytes.restype = c_size_t
     lib.mpx_fpn_forward.argtypes = [vp, vp, c_int, c_int, c_int, POINTER(vp), POINTER(vp), POINTER(vp), vp, c_size_t, vp]
+    lib.mpx_mask_paste.argtypes = [vp, vp, vp, c_int, c_int, c_int, c_int, POINTER(ctypes.c_int32), POINTER(ctypes.c_int32),
+                                   vp, POINTER(vp), vp]
     lib.mpx_bop_vsd.argtypes = [c_int, c_int, c_int, vp, c_int, vp, vp, vp, c_int, vp, c_int, vp, vp, vp, vp, vp, c_int,
                                 c_float, vp, vp, vp]
     lib.mpx_bop_point_errors.argtypes = [c_int, c_int, c_int, vp, vp, ctypes.c_longlong, vp, vp, ctypes.c_longlong, vp, vp,
@@ -110,7 +112,7 @@ EXPORTS = [
     "mpx_pose_update", "mpx_topk_per_group", "mpx_image_to_nhwc4", "mpx_roi_align", "mpx_roi_align_fused",
     "mpx_net_input_bytes", "mpx_conv2d", "mpx_conv2d_splitk", "mpx_conv_set_mode", "mpx_maxpool3x3s2", "mpx_avgpool_linear",
     "mpx_net_create", "mpx_net_create_preact", "mpx_net_destroy", "mpx_net_set_graphs", "mpx_net_workspace_bytes", "mpx_net_forward",
-    "mpx_fpn_create", "mpx_fpn_destroy", "mpx_fpn_workspace_bytes", "mpx_fpn_forward",
+    "mpx_fpn_create", "mpx_fpn_destroy", "mpx_fpn_workspace_bytes", "mpx_fpn_forward", "mpx_mask_paste",
     "mpx_bop_vsd", "mpx_bop_point_errors", "mpx_bop_gt_info",
     "mpx_teaser_points", "mpx_teaser_fps_workspace_bytes", "mpx_teaser_fps", "mpx_teaser_graph",
     "mpx_teaser_clique_workspace_bytes", "mpx_teaser_max_clique", "mpx_teaser_solve",

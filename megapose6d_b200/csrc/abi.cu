@@ -709,4 +709,37 @@ int mpx_fpn_forward(const mpx_fpn* fpn, const float* d_images, int n, int h, int
                      static_cast<cudaStream_t>(stream));
 }
 
+// ---- detector: mask inference and pasting ----
+int mpx_mask_paste(const float* d_logits, const int64_t* d_labels, const float* d_boxes, int n_masks, int n_classes,
+                   int m, int n_images, const int32_t* h_counts, const int32_t* h_sizes, float* d_boxes_out,
+                   float* const* h_masks, void* stream) {
+  MPX_REQUIRE(n_images >= 1 && n_images <= kMaskMaxImages, "mpx_mask_paste: n_images=%d, must be 1..%d", n_images,
+              kMaskMaxImages);
+  MPX_REQUIRE(n_classes >= 1 && m >= 1 && m <= kMaskMaxM, "mpx_mask_paste: n_classes=%d, m=%d: need n_classes >= 1, m 1..%d",
+              n_classes, m, kMaskMaxM);
+  MPX_REQUIRE(n_masks >= 0 && n_masks <= 65535, "mpx_mask_paste: n_masks=%d, must be 0..65535", n_masks);
+  MPX_NOT_NULL(h_counts);
+  MPX_NOT_NULL(h_sizes);
+  MPX_NOT_NULL(h_masks);
+  long long total = 0;
+  for (int i = 0; i < n_images; ++i) {
+    const int* s = h_sizes + 4 * i;
+    MPX_REQUIRE(h_counts[i] >= 0, "mpx_mask_paste: image %d has %d detections", i, h_counts[i]);
+    MPX_REQUIRE(s[0] >= 1 && s[1] >= 1 && s[2] >= 1 && s[3] >= 1 && static_cast<long long>(s[2]) * s[3] < (1ll << 31),
+                "mpx_mask_paste: image %d: sizes %dx%d -> %dx%d must be positive, H*W < 2^31", i, s[0], s[1], s[2], s[3]);
+    MPX_REQUIRE(h_counts[i] == 0 || is_device_ptr(h_masks[i]), "mpx_mask_paste: masks of image %d are NULL or not device memory",
+                i);
+    total += h_counts[i];
+  }
+  MPX_REQUIRE(total == n_masks, "mpx_mask_paste: counts add up to %lld, not n_masks=%d", total, n_masks);
+  if (n_masks > 0) {
+    MPX_DEVICE(d_logits);
+    MPX_DEVICE(d_labels);
+    MPX_DEVICE(d_boxes);
+    MPX_DEVICE(d_boxes_out);
+  }
+  return mask_paste(d_logits, reinterpret_cast<const long long*>(d_labels), d_boxes, n_masks, n_classes, m, n_images,
+                    h_counts, h_sizes, d_boxes_out, h_masks, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

@@ -6,6 +6,7 @@
 //   fpn_input_kernel     fp32 NCHW normalised image batch -> space-to-depth act16 input of the 4x4 stem
 //   fpn_resample_kernel  nearest 2x upsampling (FPN top-down path) and the stride-2 subsampling of the pool level
 //   fpn_output_kernel    act16 NHWC -> the 15 fp32 NCHW tensors torchvision's stages consume
+// After the RoI heads, mask_paste_kernel turns the mask logits of every detection into its image-sized fp32 mask.
 #include <cuda.h>
 #include <array>
 #include <vector>
@@ -398,6 +399,123 @@ int fpn_forward(Fpn* f, const float* images, int n, int h, int w, float* const* 
   MPX_CHECK_CUDA(cudaEventRecord(f->ev_out, f->side));
   MPX_CHECK_CUDA(cudaStreamWaitEvent(stream, f->ev_out, 0));
   g_launches += e->warm;
+  return MPX_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Mask inference and pasting: torchvision's maskrcnn_inference (sigmoid, the label's channel), then
+// GeneralizedRCNNTransform.postprocess: resize_boxes to the original size and paste_masks_in_image (padding 1).  Each
+// step is the fp32 operation torchvision runs, in its order, with the same roundings: the box arithmetic is written with
+// explicit round-to-nearest intrinsics (torchvision runs each of those operations as a kernel of its own, so nothing may
+// be fused into an FMA), the bilinear weights and sums as ATen's upsample_bilinear2d writes them.
+// ---------------------------------------------------------------------------------------------
+struct MaskImage {
+  float* out;               // [count, 1, H, W]
+  int start, count;         // detections start .. start + count - 1 of the batch
+  int h, w, H, W;           // transformed (model) size and original size
+};
+struct MaskPasteParams {
+  MaskImage img[kMaskMaxImages];
+  int n_images, n_classes, m;
+  float scale;              // (m + 2) / m: expand_boxes' scale, rounded to fp32 as torch rounds a Python float operand
+};
+
+// grid (pixel blocks, detection); one block pastes a slice of one detection's image-sized mask
+__global__ void __launch_bounds__(256)
+mask_paste_kernel(const __grid_constant__ MaskPasteParams p, const float* __restrict__ logits,
+                  const long long* __restrict__ labels, const float* __restrict__ boxes, float* __restrict__ boxes_out) {
+  __shared__ float prob[(kMaskMaxM + 2) * (kMaskMaxM + 2)];  // the zero-padded (m + 2)^2 probabilities
+  const int d = blockIdx.y;
+  int i = 0;
+  while (i + 1 < p.n_images && d >= p.img[i + 1].start) ++i;
+  const MaskImage im = p.img[i];
+  // resize_boxes: ratio = fp32(new) / fp32(old), then one product per coordinate
+  const float rw = __fdiv_rn(static_cast<float>(im.W), static_cast<float>(im.w));
+  const float rh = __fdiv_rn(static_cast<float>(im.H), static_cast<float>(im.h));
+  const float b0 = __fmul_rn(boxes[4 * d + 0], rw), b1 = __fmul_rn(boxes[4 * d + 1], rh);
+  const float b2 = __fmul_rn(boxes[4 * d + 2], rw), b3 = __fmul_rn(boxes[4 * d + 3], rh);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    boxes_out[4 * d + 0] = b0;
+    boxes_out[4 * d + 1] = b1;
+    boxes_out[4 * d + 2] = b2;
+    boxes_out[4 * d + 3] = b3;
+  }
+  // expand_boxes, then .to(int64) (truncation toward zero)
+  const float w_half = __fmul_rn(__fmul_rn(__fsub_rn(b2, b0), 0.5f), p.scale);
+  const float h_half = __fmul_rn(__fmul_rn(__fsub_rn(b3, b1), 0.5f), p.scale);
+  const float x_c = __fmul_rn(__fadd_rn(b2, b0), 0.5f), y_c = __fmul_rn(__fadd_rn(b3, b1), 0.5f);
+  const long long bx0 = static_cast<long long>(__fsub_rn(x_c, w_half));
+  const long long bx1 = static_cast<long long>(__fadd_rn(x_c, w_half));
+  const long long by0 = static_cast<long long>(__fsub_rn(y_c, h_half));
+  const long long by1 = static_cast<long long>(__fadd_rn(y_c, h_half));
+  // paste_mask_in_image: the (m + 2)^2 map resized to bw x bh, its pixel (x - bx0, y - by0) lands on image pixel (x, y)
+  const long long bw = bx1 - bx0 + 1 > 1 ? bx1 - bx0 + 1 : 1;
+  const long long bh = by1 - by0 + 1 > 1 ? by1 - by0 + 1 : 1;
+  const long long label = labels[d];
+  const bool valid = label >= 0 && label < p.n_classes;
+  const int mp = p.m + 2;
+  if (valid) {
+    const float* src = logits + (static_cast<size_t>(d) * p.n_classes + label) * p.m * p.m;
+    for (int k = threadIdx.x; k < mp * mp; k += blockDim.x) {
+      const int py = k / mp, px = k % mp;
+      float v = 0.f;
+      if (py >= 1 && py <= p.m && px >= 1 && px <= p.m) v = 1.0f / (1.0f + expf(-src[(py - 1) * p.m + (px - 1)]));
+      prob[k] = v;
+    }
+  }
+  __syncthreads();
+  // upsample_bilinear2d, align_corners=False, no scale factors: scale = fp32(in) / out
+  const float rheight = static_cast<float>(mp) / static_cast<float>(bh);
+  const float rwidth = static_cast<float>(mp) / static_cast<float>(bw);
+  const long long hw = static_cast<long long>(im.H) * im.W;
+  float* out = im.out + static_cast<size_t>(d - im.start) * hw;
+  for (long long k = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; k < hw;
+       k += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int y = static_cast<int>(k / im.W), x = static_cast<int>(k % im.W);
+    float val = 0.f;
+    if (valid && x >= bx0 && x <= bx1 && y >= by0 && y <= by1) {
+      const int h2 = static_cast<int>(y - by0), w2 = static_cast<int>(x - bx0);
+      float h1r = rheight * (h2 + 0.5f) - 0.5f;
+      h1r = h1r < 0.f ? 0.f : h1r;
+      const int h1 = static_cast<int>(h1r);
+      const int h1p = h1 < mp - 1 ? 1 : 0;
+      const float h1lambda = h1r - h1, h0lambda = 1.f - h1lambda;
+      float w1r = rwidth * (w2 + 0.5f) - 0.5f;
+      w1r = w1r < 0.f ? 0.f : w1r;
+      const int w1 = static_cast<int>(w1r);
+      const int w1p = w1 < mp - 1 ? 1 : 0;
+      const float w1lambda = w1r - w1, w0lambda = 1.f - w1lambda;
+      const float* r0 = prob + h1 * mp + w1;
+      const float* r1 = r0 + h1p * mp;
+      val = h0lambda * (w0lambda * r0[0] + w1lambda * r0[w1p]) + h1lambda * (w0lambda * r1[0] + w1lambda * r1[w1p]);
+    }
+    out[k] = val;
+  }
+}
+
+int mask_paste(const float* logits, const long long* labels, const float* boxes, int n_masks, int n_classes, int m,
+               int n_images, const int* counts, const int* sizes, float* boxes_out, float* const* masks,
+               cudaStream_t stream) {
+  MaskPasteParams p{};
+  p.n_images = n_images;
+  p.n_classes = n_classes;
+  p.m = m;
+  p.scale = static_cast<float>(static_cast<double>(m + 2) / m);
+  long long max_hw = 0;
+  int start = 0;
+  for (int i = 0; i < n_images; ++i) {
+    p.img[i] = MaskImage{masks[i], start, counts[i], sizes[4 * i], sizes[4 * i + 1], sizes[4 * i + 2], sizes[4 * i + 3]};
+    start += counts[i];
+    const long long hw = static_cast<long long>(sizes[4 * i + 2]) * sizes[4 * i + 3];
+    if (counts[i] > 0 && hw > max_hw) max_hw = hw;
+  }
+  if (n_masks == 0) return MPX_OK;
+  long long bx = (max_hw + 256 * 8 - 1) / (256 * 8);  // eight pixels per thread
+  if (bx < 1) bx = 1;
+  mask_paste_kernel<<<dim3(static_cast<unsigned>(bx), static_cast<unsigned>(n_masks)), 256, 0, stream>>>(
+      p, logits, labels, boxes, boxes_out);
+  MPX_CHECK_CUDA(cudaGetLastError());
+  ++g_launches;
   return MPX_OK;
 }
 

@@ -213,6 +213,11 @@ void fpn_destroy(Fpn* fpn);
 size_t fpn_workspace_bytes(int n, int h, int w);
 int fpn_forward(Fpn* fpn, const float* images, int n, int h, int w, float* const* features, float* const* objectness,
                 float* const* deltas, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+constexpr int kMaskMaxImages = 64;  // images per mask_paste call
+constexpr int kMaskMaxM = 64;       // mask resolution (Mask R-CNN: 28)
+int mask_paste(const float* logits, const long long* labels, const float* boxes, int n_masks, int n_classes, int m,
+               int n_images, const int* counts, const int* sizes, float* boxes_out, float* const* masks,
+               cudaStream_t stream);
 
 // raster.cu
 struct MeshDb {

@@ -11,6 +11,14 @@ Weights are repacked once:
   * the 7x7/s2 stem rewritten as the 4x4 convolution over the space-to-depth input (`backbone._stem_s2d`, c_pad 16);
   * `cls_logits` (A rows) and `bbox_pred` (4A rows) merged into one 1x1 convolution of 64 rows, the rest zero;
   * every matrix rounded once to the library's 16-bit type, saturating.
+
+With `device_paste=True` the module runs the RoI heads' stages one by one (the model's box RoI pool, box head, box predictor,
+postprocess_detections, mask RoI pool, mask head and mask predictor, unchanged) and then, instead of maskrcnn_inference
+and GeneralizedRCNNTransform.postprocess, one `mpx_mask_paste` (include/mpx.h) for the whole batch: sigmoid, the label's
+channel, resize_boxes and paste_masks_in_image on the device.  torchvision pastes the masks in a Python loop with several
+host synchronisations per detection; the device paste has none, so the number of synchronisations per call no longer
+grows with the number of detections.  Boxes, labels and scores are those of `device_paste=False`; the probabilities differ
+from torchvision's by a few ulps at most (see `mask_paste`).
 """
 from __future__ import annotations
 
@@ -159,6 +167,60 @@ def level_sizes(h: int, w: int) -> List[Tuple[int, int]]:
     return sizes + [((sizes[-1][0] + 1) // 2, (sizes[-1][1] + 1) // 2)]
 
 
+MASK_MAX_RESOLUTION = 64  # mpx_mask_paste's largest m (Mask R-CNN: 28)
+MASK_MAX_IMAGES = 64      # images per mpx_mask_paste call
+
+
+def check_supported_device_paste(model: nn.Module) -> None:
+    """Raises NotImplementedError for RoI heads whose masks `device_paste=True` cannot paste on the device."""
+    from torchvision.models.detection.transform import GeneralizedRCNNTransform
+
+    if type(model.transform) is not GeneralizedRCNNTransform:
+        _refuse(f"the transform {type(model.transform).__name__}")
+    rh = model.roi_heads
+    if rh.mask_roi_pool is None or rh.mask_head is None or rh.mask_predictor is None:
+        _refuse("RoI heads without a mask branch (device_paste=True pastes masks)")
+    if rh.keypoint_roi_pool is not None or rh.keypoint_head is not None or rh.keypoint_predictor is not None:
+        _refuse("a keypoint branch")
+    size = rh.mask_roi_pool.output_size
+    size = (size, size) if isinstance(size, int) else tuple(size)
+    conv5 = getattr(rh.mask_predictor, "conv5_mask", None)
+    if (size[0] != size[1] or not isinstance(conv5, nn.ConvTranspose2d) or conv5.stride != (2, 2)
+            or conv5.kernel_size != (2, 2) or 2 * size[0] > MASK_MAX_RESOLUTION):
+        _refuse(f"a mask predictor of {size} RoIs (square pools and a 2x2/2 ConvTranspose2d to at most "
+                f"{MASK_MAX_RESOLUTION}x{MASK_MAX_RESOLUTION} masks)")
+
+
+def mask_paste(mask_logits: torch.Tensor, labels: torch.Tensor, boxes: torch.Tensor, counts: List[int],
+               image_sizes: List[Tuple[int, int]], original_sizes: List[Tuple[int, int]]
+               ) -> Tuple[List[torch.Tensor], List[torch.Tensor]]:
+    """maskrcnn_inference + resize_boxes + paste_masks_in_image on the device, in one launch for the batch.
+    mask_logits [N, classes, m, m] fp32, labels [N] int64, boxes [N, 4] fp32 in the transformed images' coordinates,
+    counts: detections per image (the rows of image 0 first).  Returns per image the resized boxes [count, 4] and the
+    fp32 masks [count, 1, H, W] at the original size."""
+    n_images = len(counts)
+    if not 1 <= n_images <= MASK_MAX_IMAGES:
+        raise ValueError(f"mask_paste: {n_images} images, must be 1..{MASK_MAX_IMAGES}")
+    n, n_classes, m, m2 = mask_logits.shape
+    if m != m2 or labels.shape != (n,) or boxes.shape != (n, 4) or sum(counts) != n:
+        raise ValueError(f"mask_paste: logits {tuple(mask_logits.shape)}, labels {tuple(labels.shape)}, boxes "
+                         f"{tuple(boxes.shape)}, counts {counts}")
+    device = mask_logits.device
+    logits = mask_logits.to(torch.float32).contiguous()
+    labels = labels.to(torch.int64).contiguous()
+    boxes = boxes.to(torch.float32).contiguous()
+    boxes_out = torch.empty_like(boxes)
+    masks = [torch.empty(c, 1, H, W, device=device) for c, (H, W) in zip(counts, original_sizes)]
+    sizes = [v for (h, w), (H, W) in zip(image_sizes, original_sizes) for v in (h, w, H, W)]
+    c_counts = (ctypes.c_int32 * n_images)(*counts)
+    c_sizes = (ctypes.c_int32 * (4 * n_images))(*sizes)
+    c_masks = (ctypes.c_void_p * n_images)(*[t.data_ptr() if t.numel() else None for t in masks])
+    _abi.check(_abi.lib().mpx_mask_paste(logits.data_ptr(), labels.data_ptr(), boxes.data_ptr(), n, n_classes, m,
+                                         n_images, c_counts, c_sizes, boxes_out.data_ptr(), c_masks,
+                                         _abi.stream_ptr()))
+    return list(boxes_out.split(counts)), masks
+
+
 class FpnEngine:
     """Owns the repacked device weights and the mpx_fpn handle.  `run(images)` returns the FPN features, objectness and
     deltas of a padded fp32 batch [n, 3, h, w] as lists of five fp32 NCHW tensors.  The tensors are the engine's own
@@ -220,8 +282,11 @@ class EngineMaskRCNN(nn.Module):
     """Called like torchvision's GeneralizedRCNN in eval mode: `module(images)` -> list of dicts(boxes, labels, scores,
     masks).  Holds the model's transform, RPN and RoI heads by reference (not as submodules: it does not own them)."""
 
-    def __init__(self, model: nn.Module, device="cuda"):
+    def __init__(self, model: nn.Module, device="cuda", device_paste: bool = False):
         super().__init__()
+        if device_paste:
+            check_supported_device_paste(model)
+        self.device_paste = device_paste
         self.engine = FpnEngine(model, device)
         self._stages = (model.transform, model.rpn, model.roi_heads)
         for attr in ("config", "cfg"):
@@ -261,13 +326,31 @@ class EngineMaskRCNN(nn.Module):
         image_list, _ = transform(images)
         features, objectness, deltas = self.heads(image_list)
         proposals = self.proposals(image_list, features, objectness, deltas)
-        detections, _ = roi_heads(features, proposals, image_list.image_sizes)
-        return transform.postprocess(detections, image_list.image_sizes, original_image_sizes)
+        if not self.device_paste:
+            detections, _ = roi_heads(features, proposals, image_list.image_sizes)
+            return transform.postprocess(detections, image_list.image_sizes, original_image_sizes)
+        return self.detect(features, proposals, image_list.image_sizes, original_image_sizes)
+
+    def detect(self, features, proposals, image_sizes, original_image_sizes) -> List[Dict[str, torch.Tensor]]:
+        """RoIHeads.forward (eval) up to the mask logits with the model's modules, then `mask_paste` in place of
+        maskrcnn_inference and GeneralizedRCNNTransform.postprocess."""
+        rh = self._stages[2]
+        box_features = rh.box_head(rh.box_roi_pool(features, proposals, image_sizes))
+        class_logits, box_regression = rh.box_predictor(box_features)
+        boxes, scores, labels = rh.postprocess_detections(class_logits, box_regression, proposals, image_sizes)
+        mask_logits = rh.mask_predictor(rh.mask_head(rh.mask_roi_pool(features, boxes, image_sizes)))
+        counts = [int(b.shape[0]) for b in boxes]
+        boxes, masks = mask_paste(mask_logits, torch.cat(labels), torch.cat(boxes), counts, image_sizes,
+                                  original_image_sizes)
+        return [dict(boxes=b, labels=l, scores=s, masks=m) for b, l, s, m in zip(boxes, labels, scores, masks)]
 
 
-def engine_model(model: nn.Module, device="cuda") -> EngineMaskRCNN:
+def engine_model(model: nn.Module, device="cuda", device_paste: bool = False) -> EngineMaskRCNN:
     """`model` (a torchvision MaskRCNN on `device`, in eval mode) with its backbone and RPN head on the engine.  Raises
     NotImplementedError, before any device work, for a structure the plan does not serve: a backbone other than the
     ResNet-50 body with FPN (returned layers 1-4, 256 channels, LastLevelMaxPool), a norm other than FrozenBatchNorm2d,
-    dilation, an RPN head with conv_depth != 1 or more than 12 anchors per location, size_divisible != 32."""
-    return EngineMaskRCNN(model, device)
+    dilation, an RPN head with conv_depth != 1 or more than 12 anchors per location, size_divisible != 32.
+    `device_paste=True` also pastes the masks on the device (`mask_paste`) and refuses, likewise, RoI heads without a mask
+    branch or with a keypoint branch, non-square mask pools, a mask predictor other than a 2x2/2 ConvTranspose2d and
+    masks larger than 64x64, and a transform other than GeneralizedRCNNTransform."""
+    return EngineMaskRCNN(model, device, device_paste)

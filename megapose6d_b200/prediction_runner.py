@@ -503,7 +503,11 @@ def main(argv: Optional[List[str]] = None) -> None:
                         "truth as detections (detection_type='detector')")
     parser.add_argument("--detector-engine", action="store_true",
                         help="run the detector's ResNet-50 FPN backbone and RPN head on the engine's convolutions")
+    parser.add_argument("--detector-device-paste", action="store_true",
+                        help="as --detector-engine, and turn the detector's mask logits into image-sized masks on the device")
     args = parser.parse_args(argv)
+    if args.detector_device_paste:
+        args.detector_engine = True
     if args.detector_engine and args.detector is None:
         parser.error("--detector-engine needs --detector")
     if bool(args.frame_dirs) == (args.bop_dataset is not None):
@@ -542,7 +546,7 @@ def main(argv: Optional[List[str]] = None) -> None:
         from .detector import load_detector
 
         pose_estimator.detector_model = load_detector(args.detector, models_root=args.models_root,
-                                                      engine=args.detector_engine)
+                                                      engine=args.detector_engine, device_paste=args.detector_device_paste)
     out = run_predictions(scene_ds, pose_estimator, cfg, save_dir=args.save_dir)
     if out["save_dir"] is not None:
         n = len(out["results"]["predictions"]["final"])

@@ -3,11 +3,15 @@
 Workload: the seeded detector of `workloads.detector.make_detector` (no trained checkpoint is available), 480x640 images,
 batch 1 and 8, with `input_resize` (480, 640) and the reference default (240, 320).  Arms:
   engine     backbone + RPN head as one mpx_fpn_forward (detector_engine.engine_model), the rest torchvision fp32
+  engine_paste  as engine, and the masks pasted on the device (engine_model(..., device_paste=True): one mpx_mask_paste)
   fp32       torchvision, TF32 off
   tf32       torchvision with torch's defaults (cuDNN convolutions in TF32)
   fp16_cl    torchvision under fp16 autocast, channels_last
 Stages: `heads` = backbone + RPN head (one mpx_fpn_forward for the engine), `rest` = anchors, proposals, RoI heads and
-postprocessing from those outputs, `detector` = the whole `Detector.get_detections`.  After a warm-up, every window times
+postprocessing from those outputs, `detector` = the whole `Detector.get_detections`.  `rest` is split, on the engine's
+head outputs, into torchvision's `proposals` (anchors, decoding, filter_proposals), `box` (box RoI pool, box head, box
+predictor, postprocess_detections), `mask` (mask RoI pool, mask head, mask predictor) and `paste` (maskrcnn_inference and
+GeneralizedRCNNTransform.postprocess), next to `paste_engine` (mpx_mask_paste).  After a warm-up, every window times
 each arm in turn (CUDA events, `--calls` calls) and the medians over `--windows` windows are reported, with the engine's
 convolution TFLOP/s (mpx_profile_enable: events around every convolution, FLOPs from the shapes), the largest per-level
 relative error of each arm's head outputs against fp32, the device name and its power limit, as one JSON line.
@@ -28,6 +32,8 @@ from pathlib import Path
 import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
+
+from torchvision.models.detection.roi_heads import maskrcnn_inference  # noqa: E402
 
 from megapose6d_b200 import _abi, detector_engine as E  # noqa: E402
 from megapose6d_b200.detector import Detector  # noqa: E402
@@ -55,6 +61,43 @@ def arm_context(arm: str):
     return contextlib.nullcontext()
 
 
+def split_stages(model, engine, image_list, batch: int):
+    """torchvision's stages after the RPN head, one by one, each fed the previous stage's outputs computed once from the
+    engine's head outputs; and the device paste on the same inputs."""
+    rh, sizes, orig = model.roi_heads, image_list.image_sizes, [(480, 640)] * batch
+    with torch.no_grad():
+        feats, o, d = engine.heads(image_list)
+        props = engine.proposals(image_list, feats, o, d)
+        cls, reg = rh.box_predictor(rh.box_head(rh.box_roi_pool(feats, props, sizes)))
+        boxes, scores, labels = rh.postprocess_detections(cls, reg, props, sizes)
+        logits = rh.mask_predictor(rh.mask_head(rh.mask_roi_pool(feats, boxes, sizes)))
+    counts = [int(b.shape[0]) for b in boxes]
+
+    def proposals():
+        with torch.no_grad():
+            return engine.proposals(image_list, feats, o, d)
+
+    def box():
+        with torch.no_grad():
+            c, r = rh.box_predictor(rh.box_head(rh.box_roi_pool(feats, props, sizes)))
+            return rh.postprocess_detections(c, r, props, sizes)
+
+    def mask():
+        with torch.no_grad():
+            return rh.mask_predictor(rh.mask_head(rh.mask_roi_pool(feats, boxes, sizes)))
+
+    def paste():
+        with torch.no_grad():
+            dets = [dict(boxes=b, labels=l, scores=s, masks=p)
+                    for b, l, s, p in zip(boxes, labels, scores, maskrcnn_inference(logits, labels))]
+            return model.transform.postprocess(dets, sizes, orig)
+
+    def paste_engine():
+        return E.mask_paste(logits, torch.cat(labels), torch.cat(boxes), counts, sizes, orig)
+
+    return dict(proposals=proposals, box=box, mask=mask, paste=paste, paste_engine=paste_engine), counts
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--windows", type=int, default=5)
@@ -68,21 +111,22 @@ def main() -> None:
         model = make_detector(resize, seed=0, device="cuda")
         cl = copy.deepcopy(model).to(memory_format=torch.channels_last)
         engine = E.engine_model(model)
+        engine_paste = E.engine_model(model, device_paste=True)
         tv = {"fp32": model, "tf32": model, "fp16_cl": cl}
         for batch in (1, 8):
             g = torch.Generator().manual_seed(batch)
             images = torch.rand(batch, 3, 480, 640, generator=g).cuda()
             obs = ObservationTensor(images, torch.eye(3).repeat(batch, 1, 1).cuda())
             image_list, _ = model.transform(list(images))
-            arms = ["engine", "fp32", "tf32", "fp16_cl"]
+            arms = ["engine", "engine_paste", "fp32", "tf32", "fp16_cl"]
             heads_out, fns = {}, {}
             for arm in arms:
-                m = engine if arm == "engine" else tv[arm]
+                m = {"engine": engine, "engine_paste": engine_paste}.get(arm) or tv[arm]
                 det = Detector(m)
 
                 def heads(arm=arm):
                     with arm_context(arm), torch.no_grad():
-                        if arm == "engine":
+                        if arm.startswith("engine"):
                             f, o, d = engine.heads(image_list)
                             return list(f.values()), o, d
                         x = image_list.tensors
@@ -99,7 +143,9 @@ def main() -> None:
                 def rest(arm=arm, feats=feats, o=o, d=d):
                     with arm_context(arm), torch.no_grad():
                         props = engine.proposals(image_list, feats, o, d)
-                        r = tv[arm] if arm != "engine" else model
+                        if arm == "engine_paste":
+                            return engine_paste.detect(feats, props, image_list.image_sizes, [(480, 640)] * batch)
+                        r = tv[arm] if not arm.startswith("engine") else model
                         dets, _ = r.roi_heads(feats, props, image_list.image_sizes)
                         return r.transform.postprocess(dets, image_list.image_sizes, [(480, 640)] * batch)
 
@@ -108,13 +154,17 @@ def main() -> None:
                         return det.get_detections(obs)
 
                 fns[arm] = dict(heads=heads, rest=rest, detector=whole)
+            fns["split"], counts = split_stages(model, engine, image_list, batch)
             for arm in arms:  # warm-up: algorithm selection, graph capture
                 for fn in fns[arm].values():
                     for _ in range(3):
                         fn()
-            times = {arm: {s: [] for s in fns[arm]} for arm in arms}
+            for fn in fns["split"].values():
+                for _ in range(3):
+                    fn()
+            times = {arm: {s: [] for s in fns[arm]} for arm in arms + ["split"]}
             for _ in range(args.windows):
-                for arm in arms:
+                for arm in arms + ["split"]:
                     for stage, fn in fns[arm].items():
                         times[arm][stage].append(timed(fn, args.calls))
             med = {arm: {s: statistics.median(v) for s, v in st.items()} for arm, st in times.items()}
@@ -132,7 +182,9 @@ def main() -> None:
                         heads_speedup_vs_fp32=med["fp32"]["heads"] / med["engine"]["heads"],
                         heads_speedup_vs_tf32=med["tf32"]["heads"] / med["engine"]["heads"],
                         heads_speedup_vs_fp16_cl=med["fp16_cl"]["heads"] / med["engine"]["heads"],
-                        detector_speedup_vs_fp32=med["fp32"]["detector"] / med["engine"]["detector"])
+                        detector_speedup_vs_fp32=med["fp32"]["detector"] / med["engine"]["detector"],
+                        detector_speedup_paste_vs_engine=med["engine"]["detector"] / med["engine_paste"]["detector"],
+                        detections=counts)
             out["cases"].append(case)
             print(json.dumps(case), file=sys.stderr, flush=True)
     print(json.dumps(out))
