@@ -156,6 +156,8 @@ int mpx_render_crop_fused(const mpx_meshdb* db, const int32_t* d_label_idx, cons
 /* ---- hypothesis geometry -----------------------------------------------------------------------
  * mpx_pose_init_autodepth: TCO_init_from_boxes_autodepth_with_R (lib3d/cosypose_ops.py:169-218).
  *   d_points [n_labels, n_pts, 3]; d_label_idx, d_bboxes [n,4], d_K [n,9], d_R [n,9] -> d_TCO [n,16]
+ *   n_pts > 0.  Non-finite inputs propagate as in torch: a NaN model point coordinate (R, box or K NaN) makes the
+ *   extent and so the translation NaN; x2 = x1 - 1 (bb_dx = 0) gives an infinite depth, as in the reference.
  */
 int mpx_pose_init_autodepth(const float* d_points, int n_pts, const int32_t* d_label_idx,
                             const float* d_bboxes, const float* d_K, const float* d_R, int n,
@@ -169,7 +171,10 @@ int mpx_normalize_T(const float* d_T_in, int n, float* d_T_out, void* stream);
  * boxes_from_uv (lib3d/camera_geometry.py:40-64), deepim_boxes via deepim_crops_robust
  * (lib3d/cropping.py:30-110), get_K_crop_resize (lib3d/camera_geometry.py:67-115).
  *   d_points [n_labels, n_pts, 3] (the deterministic 2000- or 200-point subsets)
- *   d_tCR [n,3]; outputs d_boxes_rend [n,4], d_boxes_crop [n,4], d_K_crop [n,9] */
+ *   d_tCR [n,3]; outputs d_boxes_rend [n,4], d_boxes_crop [n,4], d_K_crop [n,9].  n_pts > 0, sizes > 0.
+ *   NaN propagates as in torch: the 0.1 z clamps, the box min / max and deepim's maxima return NaN for a NaN operand,
+ *   and a non-finite row of K @ R makes that coordinate of the rendering centre NaN (the reference projects the origin
+ *   through K @ [R | tCR]).  A NaN pose gives NaN boxes and NaN K_crop entries with the zeros and the 1 kept. */
 int mpx_crop_geometry(const float* d_points, int n_pts, const int32_t* d_label_idx,
                       const float* d_TCO, const float* d_K, const float* d_tCR, int n, float lamb,
                       int im_h, int im_w, int out_h, int out_w, float* d_boxes_rend,
@@ -178,7 +183,8 @@ int mpx_crop_geometry(const float* d_points, int n_pts, const int32_t* d_label_i
 /* mpx_multiview_cameras: make_TCO_multiview (lib3d/multiview.py:165-246), closed form of the
  * Panda3D scene-graph look-at (multiview.py:31-92); float64 internally.
  *   h_offsets [n_extra,3] camera positions wrt camera 0 in units of |tCR|
- *   d_TCV_O [n, 1 + n_extra, 16]: view 0 is TCO itself */
+ *   d_TCV_O [n, 1 + n_extra, 16]: view 0 is TCO itself.  0 <= n_extra <= 32.  A non-finite TCO takes the
+ *   reference's identity fallback (multiview.py:44-46); its extra views come out NaN, as in the closed form. */
 int mpx_multiview_cameras(const float* d_TCO, const float* d_tCR, int n, const float* h_offsets,
                           int n_extra, float* d_TCV_O, void* stream);
 
@@ -191,7 +197,8 @@ int mpx_pose_update(const float* d_TCO, const float* d_K_crop, const float* d_po
 /* mpx_topk_per_group: top-K by logit per detection, the device-side equivalent of
  * PoseEstimator.filter_pose_estimates (inference/pose_estimator.py:643-667) for the coarse
  * stage.  d_logits [n_groups, m]; d_idx [n_groups, k] int32 indices into m, descending logit,
- * ties broken by lower index. */
+ * ties broken by lower index (-0 ties +0), NaN after every number including -inf: the order of
+ * sort_values(ascending=False).  k <= m <= 12000; n_groups == 0 or k == 0 launches nothing. */
 int mpx_topk_per_group(const float* d_logits, int n_groups, int m, int k, int32_t* d_idx,
                        void* stream);
 

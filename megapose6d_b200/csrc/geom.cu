@@ -6,6 +6,8 @@
 //            lib3d/cropping.py:30-110; lib3d/transform_ops.py:106-119; lib3d/rotations.py:25-40;
 //            lib3d/multiview.py:31-92,165-246; models/pose_rigid.py:180-303,305-312;
 //            inference/pose_estimator.py:643-667.
+#include <climits>
+
 #include "mpx_common.cuh"
 
 namespace mpx {
@@ -13,11 +15,25 @@ namespace mpx {
 // ---------------------------------------------------------------------------------------------
 // block-wide min/max helpers (blockDim.x multiple of 32, <= 1024)
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void block_minmax4(float& mn0, float& mx0, float& mn1, float& mx1, float* sm) {
+// fminf/fmaxf drop NaN; torch's min/max reductions and torch.max(a, b) return it.  The reductions below keep the fast
+// fminf/fmaxf and carry an "any NaN" bit per coordinate instead (bit 0: coordinate 0, bit 1: coordinate 1); a flagged
+// coordinate's min and max are NaN, as torch computes them.
+__device__ __forceinline__ unsigned nan_bits(float c0, float c1) {
+  return (c0 != c0 ? 1u : 0u) | (c1 != c1 ? 2u : 0u);
+}
+// torch.max(a, b) (elementwise): NaN if either operand is NaN, fmaxf otherwise
+__device__ __forceinline__ float max_nan(float a, float b) { return a != a ? a : (b != b ? b : fmaxf(a, b)); }
+
+__device__ __forceinline__ void block_minmax4(float& mn0, float& mx0, float& mn1, float& mx1, unsigned nan, float* sm) {
+  __shared__ unsigned s_nan;
+  if (threadIdx.x == 0) s_nan = 0u;
   mn0 = warp_min(mn0); mx0 = warp_max(mx0); mn1 = warp_min(mn1); mx1 = warp_max(mx1);
+  nan = __reduce_or_sync(0xffffffffu, nan);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  __syncthreads();  // s_nan cleared before any warp adds to it
   if (lane == 0) {
     sm[warp * 4 + 0] = mn0; sm[warp * 4 + 1] = mx0; sm[warp * 4 + 2] = mn1; sm[warp * 4 + 3] = mx1;
+    if (nan) atomicOr(&s_nan, nan);
   }
   __syncthreads();
   if (warp == 0) {
@@ -26,7 +42,12 @@ __device__ __forceinline__ void block_minmax4(float& mn0, float& mx0, float& mn1
     float c = lane < nw ? sm[lane * 4 + 2] : INFINITY;
     float d = lane < nw ? sm[lane * 4 + 3] : -INFINITY;
     a = warp_min(a); b = warp_max(b); c = warp_min(c); d = warp_max(d);
-    if (lane == 0) { sm[0] = a; sm[1] = b; sm[2] = c; sm[3] = d; }
+    if (lane == 0) {
+      const unsigned f = s_nan;
+      if (f & 1u) a = b = NAN;
+      if (f & 2u) c = d = NAN;
+      sm[0] = a; sm[1] = b; sm[2] = c; sm[3] = d;
+    }
   }
   __syncthreads();
   mn0 = sm[0]; mx0 = sm[1]; mn1 = sm[2]; mx1 = sm[3];
@@ -49,14 +70,16 @@ __global__ void pose_init_kernel(const float* __restrict__ points, int n_pts, co
   const float tx = ((bcx - cx) * z_guess) / fx, ty = ((bcy - cy) * z_guess) / fy;
   const float* pts = points + static_cast<size_t>(label_idx[n]) * n_pts * 3;
   float mnx = INFINITY, mxx = -INFINITY, mny = INFINITY, mxy = -INFINITY;
+  unsigned nan = 0u;
   for (int i = threadIdx.x; i < n_pts; i += blockDim.x) {
     const float px = __ldg(pts + 3 * i), py = __ldg(pts + 3 * i + 1), pz = __ldg(pts + 3 * i + 2);
     const float x = Rn[0] * px + Rn[1] * py + Rn[2] * pz + tx;
     const float y = Rn[3] * px + Rn[4] * py + Rn[5] * pz + ty;
     mnx = fminf(mnx, x); mxx = fmaxf(mxx, x);
     mny = fminf(mny, y); mxy = fmaxf(mxy, y);
+    nan |= nan_bits(x, y);
   }
-  block_minmax4(mnx, mxx, mny, mxy, sm);
+  block_minmax4(mnx, mxx, mny, mxy, nan, sm);
   if (threadIdx.x == 0) {
     const float deltax = mxx - mnx, deltay = mxy - mny;
     const float bb_dx = (bb[2] - bb[0]) + 1.f, bb_dy = (bb[3] - bb[1]) + 1.f;
@@ -146,35 +169,41 @@ __global__ void crop_geometry_kernel(const float* __restrict__ points, int n_pts
   __syncthreads();
   const float* pts = points + static_cast<size_t>(label_idx[n]) * n_pts * 3;
   float mnu = INFINITY, mxu = -INFINITY, mnv = INFINITY, mxv = -INFINITY;
+  unsigned nan = 0u;
   for (int i = threadIdx.x; i < n_pts; i += blockDim.x) {
     const float px = __ldg(pts + 3 * i), py = __ldg(pts + 3 * i + 1), pz = __ldg(pts + 3 * i + 2);
     const float su = P[0] * px + P[1] * py + P[2] * pz + P[3];
     const float sv = P[4] * px + P[5] * py + P[6] * pz + P[7];
     float sz = P[8] * px + P[9] * py + P[10] * pz + P[11];
-    sz = fmaxf(0.1f, sz);
+    sz = max_nan(0.1f, sz);
     const float u = su / sz, v = sv / sz;
     mnu = fminf(mnu, u); mxu = fmaxf(mxu, u);
     mnv = fminf(mnv, v); mxv = fmaxf(mxv, v);
+    nan |= nan_bits(u, v);
   }
-  block_minmax4(mnu, mxu, mnv, mxv, sm);
+  block_minmax4(mnu, mxu, mnv, mxv, nan, sm);
   if (threadIdx.x == 0) {
     const float x1 = mnu, y1 = mnv, x2 = mxu, y2 = mxv;
     float* br = boxes_rend + 4 * n;
     br[0] = x1; br[1] = y1; br[2] = x2; br[3] = y2;
-    // reference point projection: K @ tCR, z clamped
+    // reference point projection: K @ tCR, z clamped.  The reference projects the origin through K @ [R | tCR], so a
+    // non-finite entry of row r of K @ R reaches row r of its result as inf * 0 = NaN (or NaN * 0)
     const float* tr = tCR + 3 * n;
-    const float cu = Kn[0] * tr[0] + Kn[1] * tr[1] + Kn[2] * tr[2];
-    const float cv = Kn[3] * tr[0] + Kn[4] * tr[1] + Kn[5] * tr[2];
+    float cu = Kn[0] * tr[0] + Kn[1] * tr[1] + Kn[2] * tr[2];
+    float cv = Kn[3] * tr[0] + Kn[4] * tr[1] + Kn[5] * tr[2];
     float cz = Kn[6] * tr[0] + Kn[7] * tr[1] + Kn[8] * tr[2];
-    cz = fmaxf(0.1f, cz);
+    if (!(isfinite(P[0]) && isfinite(P[1]) && isfinite(P[2]))) cu = NAN;
+    if (!(isfinite(P[4]) && isfinite(P[5]) && isfinite(P[6]))) cv = NAN;
+    if (!(isfinite(P[8]) && isfinite(P[9]) && isfinite(P[10]))) cz = NAN;
+    cz = max_nan(0.1f, cz);
     const float xc = cu / cz, yc = cv / cz;
-    // deepim_boxes with obs_boxes == rend_boxes (pose_rigid.py:218-229)
+    // deepim_boxes with obs_boxes == rend_boxes (pose_rigid.py:218-229); torch.max propagates NaN
     const float wmax = static_cast<float>(max(im_h, im_w)), hmin = static_cast<float>(min(im_h, im_w));
     const float r = static_cast<float>(static_cast<double>(wmax) / static_cast<double>(hmin));
-    const float xdist = fmaxf(fabsf(x1 - xc), fabsf(x2 - xc));
-    const float ydist = fmaxf(fabsf(y1 - yc), fabsf(y2 - yc));
-    const float width = fmaxf(xdist, ydist * r) * 2.f * lamb;
-    const float height = fmaxf(xdist / r, ydist) * 2.f * lamb;
+    const float xdist = max_nan(fabsf(x1 - xc), fabsf(x2 - xc));
+    const float ydist = max_nan(fabsf(y1 - yc), fabsf(y2 - yc));
+    const float width = max_nan(xdist, ydist * r) * 2.f * lamb;
+    const float height = max_nan(xdist / r, ydist) * 2.f * lamb;
     const float bx1 = xc - width / 2.f, by1 = yc - height / 2.f;
     const float bx2 = xc + width / 2.f, by2 = yc + height / 2.f;
     float* bc = boxes_crop + 4 * n;
@@ -356,50 +385,54 @@ int pose_update(const float* TCO, const float* K_crop, const float* pose9, const
 // ---------------------------------------------------------------------------------------------
 // top-K per detection (pose_estimator.py:643-667 for the coarse stage); one CTA per group
 // ---------------------------------------------------------------------------------------------
+// Logits are compared as order-preserving integer keys: a float's bits with the magnitude bits flipped when negative, -0
+// taken as +0 (a tie, as in every sort).  NaN gets a key below -inf's, so it sorts after every number (pandas
+// sort_values(ascending=False), numpy argsort of -x), and an entry already selected gets the lowest key of all.
+constexpr int kTopkNanKey = INT_MIN + 1;
+constexpr int kTopkTakenKey = INT_MIN;
+__device__ __forceinline__ int topk_key(float v) {
+  if (v != v) return kTopkNanKey;
+  const int b = __float_as_int(v == 0.f ? 0.f : v);
+  return b >= 0 ? b : b ^ 0x7fffffff;
+}
+
 __global__ void topk_kernel(const float* __restrict__ logits, int m, int k, int* __restrict__ idx) {
-  extern __shared__ float vals[];  // [m]
-  __shared__ float s_best[32];
+  extern __shared__ int keys[];  // [m]
+  __shared__ int s_best[32];
   __shared__ int s_idx[32];
   const int g = blockIdx.x;
-  for (int i = threadIdx.x; i < m; i += blockDim.x) {
-    float v = logits[static_cast<size_t>(g) * m + i];
-    vals[i] = (v == v) ? v : -INFINITY;  // NaN sorts last
-  }
+  for (int i = threadIdx.x; i < m; i += blockDim.x) keys[i] = topk_key(logits[static_cast<size_t>(g) * m + i]);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  // every untaken entry has a key above kTopkTakenKey, and k <= m leaves one untaken: each round selects a real entry,
+  // the highest key with ties to the lowest index
   for (int sel = 0; sel < k; ++sel) {
-    float best = -INFINITY;
+    int best = kTopkTakenKey;
     int bi = 0x7fffffff;
     for (int i = threadIdx.x; i < m; i += blockDim.x) {
-      const float v = vals[i];
+      const int v = keys[i];
       if (v > best || (v == best && i < bi)) { best = v; bi = i; }
     }
-    // a consumed entry is marked with NaN and never selected again
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
-      const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+      const int ob = __shfl_xor_sync(0xffffffffu, best, o);
       const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
       if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
     }
     if (lane == 0) { s_best[warp] = best; s_idx[warp] = bi; }
     __syncthreads();
     if (warp == 0) {
-      best = lane < nw ? s_best[lane] : -INFINITY;
+      best = lane < nw ? s_best[lane] : kTopkTakenKey;
       bi = lane < nw ? s_idx[lane] : 0x7fffffff;
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
-        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+        const int ob = __shfl_xor_sync(0xffffffffu, best, o);
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
         if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
       }
       if (lane == 0) {
-        if (bi == 0x7fffffff) {
-          // all remaining entries are -inf/NaN: take the lowest unconsumed index
-          for (int i = 0; i < m; ++i)
-            if (!(vals[i] != vals[i])) { bi = i; break; }
-        }
         idx[static_cast<size_t>(g) * k + sel] = bi;
-        if (bi != 0x7fffffff) vals[bi] = NAN;
+        keys[bi] = kTopkTakenKey;
       }
     }
     __syncthreads();

@@ -27,6 +27,25 @@ from .tensor_collection import PandasTensorCollection
 from .types import DetectionsType, ObservationTensor, PoseEstimatesType, assert_detections_valid
 
 
+def order_desc_nan_last(x: torch.Tensor) -> torch.Tensor:
+    """Indices that sort the 1-D `x` by descending value with NaN last and ties in index order, as the reference's
+    `sort_values(ascending=False)` orders its rows (and `filter_pose_estimates` on the host).  torch.sort alone puts NaN
+    first: NaN is sorted as -inf here, then moved behind the real -inf entries by a second stable sort."""
+    nan = torch.isnan(x)
+    order = torch.sort(torch.where(nan, torch.full_like(x, float("-inf")), x), descending=True, stable=True).indices
+    return order[torch.sort(nan[order].to(torch.int32), stable=True).indices]
+
+
+def best_per_group(logits: torch.Tensor, group: torch.Tensor, n_groups: int) -> torch.Tensor:
+    """Rows of `sort_values(logit, ascending=False).groupby(group).head(1)`, in that order: each group's best row (NaN
+    last, ties to the lower row), groups ordered by the position of their best row.  Every group must own a row."""
+    order = order_desc_nan_last(logits)
+    pos = torch.arange(logits.numel(), device=logits.device)
+    first = torch.full((n_groups,), logits.numel(), device=logits.device, dtype=torch.long)
+    first.scatter_reduce_(0, group[order], pos, "amin")
+    return order[torch.sort(first).values]
+
+
 def add_instance_id(inputs):
     """inference/utils.py:151-171: unique id per (batch_im_id, label) occurrence."""
     if "instance_id" in inputs.infos:
@@ -422,15 +441,15 @@ class PoseEstimator(torch.nn.Module):
                     out=dict(render_time=timing["render"], model_time=timing["model"]))
 
     def _coarse_select(self, st: dict, logits: torch.Tensor, rows_c: dict, B: int, M: int, Kh: int) -> dict:
-        """Scores and the top-K rows per detection, ordered like `sort_values(descending).groupby().head(K)`, on the
-        device; `logits` are the gathered logits of all B*M rows."""
+        """Scores and the top-K rows per detection, ordered like `sort_values(descending).groupby().head(K)` (NaN last,
+        ties to the lower row), on the device; `logits` are the gathered logits of all B*M rows."""
         batch_im_ids, label_idx = rows_c["batch_im_ids"], rows_c["label_idx"]
         K_rows, bboxes, TCO = st["K_rows"], st["bboxes"], st["TCO"]
         scores = torch.sigmoid(logits)
         flat = logits.flatten()
         top = lib3d.topk_per_group(logits.reshape(B, M), Kh).long()                       # [B, Kh]
         rows = (top + rows_c["group_base"]).flatten()
-        rows = rows[torch.sort(flat[rows], descending=True, stable=True).indices]
+        rows = rows[order_desc_nan_last(flat[rows])]
         packed_c = torch.cat((flat.double(), scores.flatten().double(), rows.double()))
         return dict(K_rows=K_rows, bboxes=bboxes, TCO=TCO, logits=logits, scores=scores, rows=rows, packed_c=packed_c,
                     TCO_sel=TCO[rows], bim_sel=batch_im_ids[rows], lab_sel=label_idx[rows], K_sel=K_rows[rows],
@@ -647,11 +666,7 @@ class PoseEstimator(torch.nn.Module):
         # ---- best hypothesis per detection, ordered like sort_values(pose_logit, descending).groupby().head(1)
         pl = pose_logits.flatten()
         grp = torch.div(rows, M, rounding_mode="floor")
-        order = torch.sort(pl, descending=True, stable=True).indices           # all rows by descending pose logit
-        g_sorted = grp[order]
-        pos = torch.arange(n_sel, device=device)
-        first = torch.full((B,), n_sel, device=device, dtype=torch.long).scatter_reduce_(0, g_sorted, pos, "amin")
-        keep = order[torch.sort(first).values]                                 # [B] rows of the scored collection
+        keep = best_per_group(pl, grp, B)                                      # [B] rows of the scored collection
         if st["static"]:
             main.wait_event(self.__dict__["_coarse_copies_done"])  # the side-stream clones (K_sel ...) are read from here on
         final_tensors = {k: v[keep] for k, v in refined[-1].items()} if n_refiner_iterations > 0 else None
