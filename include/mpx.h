@@ -271,6 +271,13 @@ int mpx_conv2d_splitk(const void* d_x, int n, int h, int w, int c_in, const void
  *       whose C_in is at most 128 loads one band of whole input rows per (filter row, 64 channels) instead and reuses
  *       it over the filter's columns; the outputs are identical
  *   67108864 (bit 26) use the pixel-major C_out = 64 kernel for every convolution it can serve, whatever its size
+ *   134217728 (bit 27) never use the ping-pong kernel (the 128-row kernel serves those convolutions).  By default a
+ *       convolution with C_out = 128 and at least 2 * mpx_sm_count() 128-row tiles (automatic tile width, no K split, no
+ *       pooled epilogue) runs on it: each of two consumer warpgroups owns a whole 128 x 128 tile, they take alternate
+ *       tiles so one's epilogue overlaps the other's MMAs, and the epilogue is staged through shared memory and stored by
+ *       TMA; the outputs are identical
+ *   268435456 (bit 28) use the ping-pong kernel for every convolution it can serve (C_out a multiple of 128 up to 512),
+ *       whatever its size
  * Other bits are accepted and have no effect. */
 int mpx_conv_set_mode(int mode);
 

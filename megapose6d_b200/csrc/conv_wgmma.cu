@@ -941,6 +941,211 @@ conv64_wgmma_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_cons
 }
 
 // ---------------------------------------------------------------------------------------------
+// C_out = 128 .. 512: ping-pong consumers that each own a whole 128 x 128 tile, and a TMA epilogue
+// ---------------------------------------------------------------------------------------------
+// The producer is conv_wgmma_kernel<128>'s (one 128 x 64 im2col box and one 128 x 64 weight box per k-block; items in
+// (m-tile, n-tile) order, n fastest, so consecutive items reuse the activation box from L2).  Warpgroups 1 and 2 take
+// alternate items of the CTA's persistent sequence: per k16 step one warpgroup issues two m64n128k16 (rows 0-63 and 64-127)
+// with the same B descriptor, 128 fp32 accumulators per thread, and hands the mainloop to the other warpgroup when its
+// last k-block is issued, so one runs its epilogue while the other keeps the tensor pipe busy.  Epilogue as in
+// conv64_wgmma_kernel: the residual is TMA-loaded into the warpgroup's staging tile (two 128 x 64 boxes, 128B swizzle)
+// while the mainloop runs, bias + residual + ReLU + conversion overwrite it in place, and two TMA stores write it out
+// (rows >= M_total clipped by the tensor map).  Every output's k16 sum order is that of conv_wgmma_kernel.
+constexpr int kPPStages = 4;
+constexpr int kPPStageBytes = 2 * kATileBytes;            // 16 KiB activations + 16 KiB weights
+constexpr int kPPStagingBytes = kBlockM * 128 * 2;        // 32 KiB per consumer warpgroup
+constexpr int kPPBufferBytes = kPPStages * kPPStageBytes + 2 * kPPStagingBytes;
+constexpr int kPPSmemBytes = kPPBufferBytes + 1024 /*align slack*/ + 256 /*barriers*/ + 2048 /*bias, C_out <= 512*/;
+
+struct ConvPPParams {
+  int P, Q, S, stride, pad_h, pad_w, cblocks, num_k_blocks, m_tiles, n_tiles;
+  int relu;
+  int has_residual;
+  const float* bias;
+};
+
+__global__ void __launch_bounds__(kThreads, 1)
+convpp_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                    const __grid_constant__ CUtensorMap map_res, const __grid_constant__ CUtensorMap map_out,
+                    const ConvPPParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + kPPStages * kATileBytes;
+  uint8_t* staging = smem + kPPStages * kPPStageBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kPPBufferBytes);
+  uint64_t* full_bar = bars;       // [kPPStages]
+  uint64_t* empty_bar = bars + 8;  // [kPPStages]
+  uint64_t* res_bar = bars + 16;   // [2], one per consumer warpgroup
+  float* bias_s = reinterpret_cast<float*>(bars + 32);
+
+  const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);
+  const int nk = p.num_k_blocks;
+  const int items = p.m_tiles * p.n_tiles;
+  for (int i = threadIdx.x; i < 128 * p.n_tiles; i += blockDim.x) bias_s[i] = p.bias[i];
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_out) : "memory");
+    if (p.has_residual) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_res) : "memory");
+    for (int i = 0; i < kPPStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 4);  // one arrive per warp of the consuming warpgroup
+    }
+    mbar_init(&res_bar[0], 1);
+    mbar_init(&res_bar[1], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  pdl_trigger();
+  __syncthreads();
+  pdl_wait();
+
+  if (wg == 0) {
+    // ===================== TMA producer =====================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      const int pq = p.P * p.Q;
+      for (int item = blockIdx.x; item < items; item += gridDim.x) {
+        const int m_tile = item / p.n_tiles;
+        const int n_tile = item - m_tile * p.n_tiles;
+        const int m0 = m_tile * kBlockM;
+        const int img = m0 / pq;
+        const int rem = m0 - img * pq;
+        const int p0 = rem / p.Q;
+        const int q0 = rem - p0 * p.Q;
+        const int base_w = q0 * p.stride - p.pad_w;
+        const int base_h = p0 * p.stride - p.pad_h;
+        int tap = 0, cb = 0;
+        for (int kb = 0; kb < nk; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1u);
+          mbar_expect_tx(&full_bar[stage], kPPStageBytes);
+          const int r = tap / p.S;
+          const int s = tap - r * p.S;
+          tma_load_im2col_4d(smem_a + stage * kATileBytes, &map_a, &full_bar[stage], cb * kBlockK, base_w, base_h, img,
+                             static_cast<uint16_t>(s), static_cast<uint16_t>(r));
+          tma_load_2d(smem_b + stage * kATileBytes, &map_b, &full_bar[stage], kb * kBlockK, n_tile * 128);
+          if (++cb == p.cblocks) {
+            cb = 0;
+            ++tap;
+          }
+          if (++stage == kPPStages) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
+      }
+    }
+  } else {
+    // ===================== consumers: wgmma + staged epilogue =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = wg - 1;
+    const int t = threadIdx.x & 127;
+    const int lane = threadIdx.x & 31;
+    const int row0 = 16 * (t >> 5) + (lane >> 2);  // + 64 mh + 8 h: the accumulator rows of this thread
+    const int col = 2 * (lane & 3);                 // + 8 j: its column pair
+    uint8_t* stage_buf = staging + cw * kPPStagingBytes;
+    int local = 0;
+    for (int i = cw, item = blockIdx.x + cw * gridDim.x; item < items; i += 2, item += 2 * gridDim.x, ++local) {
+      const int m_tile = item / p.n_tiles;
+      const int n0 = (item - m_tile * p.n_tiles) * 128;
+      const int m0 = m_tile * kBlockM;
+      if (p.has_residual && t == 0) {
+        bulk_wait_read_all();  // the previous item's store has read the staging tile
+        mbar_expect_tx(&res_bar[cw], kPPStagingBytes);
+        tma_load_2d(stage_buf, &map_res, &res_bar[cw], n0, m0);
+        tma_load_2d(stage_buf + kPPStagingBytes / 2, &map_res, &res_bar[cw], n0 + 64, m0);
+      }
+      // stage / phase from the CTA's k-block counter (both warpgroups' items, in item order), as in conv64_wgmma_kernel
+      const uint32_t g = static_cast<uint32_t>(i) * static_cast<uint32_t>(nk);
+      int stage = static_cast<int>(g % kPPStages);
+      uint32_t phase = (g / kPPStages) & 1u;
+      float acc0[64], acc1[64];  // rows 0-63 / 64-127 of the tile
+#pragma unroll
+      for (int j = 0; j < 64; ++j) {
+        acc0[j] = 0.f;
+        acc1[j] = 0.f;
+      }
+      // mainloop hand-off: see conv64_wgmma_kernel
+      if (i > 0) mainloop_turn_wait(cw);
+      int prev_stage = -1;
+#pragma unroll 1
+      for (int kb = 0; kb < nk; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t da = make_sw128_desc(smem_u32(smem_a + stage * kATileBytes));
+        const uint64_t db = make_sw128_desc(smem_u32(smem_b + stage * kATileBytes));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) {  // 64 rows of 128 B = 8 KiB: +512 in the (addr >> 4) field
+          wgmma_m64n128k16(acc0, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), 1u);
+          wgmma_m64n128k16(acc1, da + static_cast<uint64_t>(512 + 2 * k), db + static_cast<uint64_t>(2 * k), 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage can be refilled
+        __syncwarp();
+        if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+        prev_stage = stage;
+        if (++stage == kPPStages) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
+      if (item + static_cast<int>(gridDim.x) < items) mainloop_turn_pass(cw);
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+      if (t == 0) bulk_wait_read_all();
+      warpgroup_sync(cw);
+      if (p.has_residual) mbar_wait(&res_bar[cw], static_cast<uint32_t>(local) & 1u);
+      // staging tile: box c / 64 holds channels n0 + 64 (c / 64) .., row m at 128 m, 16-byte chunk k of the row at
+      // (k ^ (m & 7)) * 16 (128B swizzle); a warp's 8 rows x 4 lanes hit 32 distinct banks
+      const uint32_t sbase = smem_u32(stage_buf);
+#pragma unroll
+      for (int mh = 0; mh < 2; ++mh) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = 64 * mh + row0 + 8 * h;
+          const uint32_t rbase = sbase + static_cast<uint32_t>(row * 128 + col * 2);
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const float2 b = *reinterpret_cast<const float2*>(bias_s + n0 + 8 * j + col);
+            const float v0 = mh ? acc1[4 * j + 2 * h] : acc0[4 * j + 2 * h];
+            const float v1 = mh ? acc1[4 * j + 2 * h + 1] : acc0[4 * j + 2 * h + 1];
+            float f0 = v0 + b.x;
+            float f1 = v1 + b.y;
+            const uint32_t addr = rbase + static_cast<uint32_t>((j >> 3) * (kPPStagingBytes / 2) +
+                                                                (((j & 7) ^ (row & 7)) << 4));
+            if (p.has_residual) {
+              uint32_t rr;
+              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(rr) : "r"(addr) : "memory");
+              const float2 r = unpack_act2(rr);
+              f0 += r.x;
+              f1 += r.y;
+            }
+            if (p.relu) {
+              f0 = fmaxf(f0, 0.f);
+              f1 = fmaxf(f1, 0.f);
+            }
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_act2(f0, f1)) : "memory");
+          }
+        }
+      }
+      fence_proxy_async_smem();
+      warpgroup_sync(cw);
+      if (t == 0) {
+        tma_store_2d(&map_out, stage_buf, n0, m0);
+        tma_store_2d(&map_out, stage_buf + kPPStagingBytes / 2, n0 + 64, m0);
+        bulk_commit();
+      }
+    }
+    if (t == 0) bulk_wait_all();
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Host side: tensor maps + launch
 // ---------------------------------------------------------------------------------------------
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
@@ -1181,6 +1386,51 @@ static int conv64_forward(const ConvDesc& d, const void* x, const void* w, const
   return MPX_OK;
 }
 
+static int convpp_forward(const ConvDesc& d, const void* x, const void* w, const float* bias, const void* residual,
+                          void* out, int M_total, int P, int Q, int cap, cudaStream_t stream) {
+  ConvPPParams p{};
+  p.P = P;
+  p.Q = Q;
+  p.S = d.S;
+  p.stride = d.stride;
+  p.pad_h = d.pad_lo_h;
+  p.pad_w = d.pad_lo_w;
+  p.cblocks = d.C_in / kBlockK;
+  p.num_k_blocks = d.R * d.S * p.cblocks;
+  p.m_tiles = (M_total + kBlockM - 1) / kBlockM;
+  p.n_tiles = d.C_out / 128;
+  p.relu = d.relu;
+  p.has_residual = residual != nullptr;
+  p.bias = bias;
+  CUtensorMap map_a, map_b, map_res, map_out;
+  int rc = encode_im2col_map(&map_a, d, x);
+  if (rc != MPX_OK) return rc;
+  rc = encode_2d_map(&map_b, w, static_cast<cuuint64_t>(p.num_k_blocks) * kBlockK, d.C_out, kBlockK, 128,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
+  if (rc != MPX_OK) return rc;
+  rc = encode_2d_map(&map_out, out, d.C_out, M_total, 64, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+  if (rc != MPX_OK) return rc;
+  map_res = map_out;
+  if (residual != nullptr) {
+    rc = encode_2d_map(&map_res, residual, d.C_out, M_total, 64, kBlockM, CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
+    if (rc != MPX_OK) return rc;
+  }
+  static bool attr_set = false;
+  if (!attr_set) {
+    MPX_CHECK_CUDA(cudaFuncSetAttribute(convpp_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPPSmemBytes));
+    attr_set = true;
+  }
+  const int items = p.m_tiles * p.n_tiles;
+  const int grid = items < cap ? items : cap;
+  ProfileSlot* slot = profile_begin(stream);
+  MPX_CHECK_CUDA(launch_pdl(convpp_wgmma_kernel, dim3(grid), dim3(kThreads), kPPSmemBytes, stream, 1, map_a, map_b,
+                            map_res, map_out, p));
+  MPX_CHECK_CUDA(cudaGetLastError());
+  ++g_launches;
+  profile_end(slot, stream, 2.0 * M_total * d.C_out * p.num_k_blocks * kBlockK);
+  return MPX_OK;
+}
+
 // x: [n_img, H, W, C_in] act16; w: [C_out, R*S*C_in] act16 ((r,s,c) ordered); bias fp32 [C_out];
 // residual/out: [n_img, P, Q, C_out] act16.
 int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* bias,
@@ -1229,6 +1479,19 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
     const int nkb = d.R * d.S * (d.C_in / kBlockK);
     if (!(splitk < 0 && m_tiles128 * 2 <= cap && nkb >= 8))
       return conv64_forward(d, x, w, bias, residual, out, static_cast<int>(M_total), P, Q, cap, stream);
+  }
+
+  // C_out = 128 with at least two 128 x 128 tiles per CTA: the ping-pong kernel.  C_out = 256 and 512 keep the 128 x 256
+  // tiles of the 128-row kernel by default: a 128-wide tile fills 32 KB of shared memory per 128 x 128 x 64 block where
+  // those fill 48 KB per twice the work, and on an H100 that costs the 3x3 convolutions of layers 3 and 4 more than the
+  // overlapped epilogue gains (DESIGN 3.1).  Mode bit 27 never takes it, bit 28 takes it for every C_out it serves
+  // (multiples of 128 up to 512), whatever the size, except for a shape the small-batch heuristic splits over K.
+  const long long m_tiles = (M_total + kBlockM - 1) / kBlockM;
+  if (d.C_out % 128 == 0 && d.C_out <= 512 && block_n_override == 0 && splitk <= 0 && !d.pool && aligned &&
+      (g_conv_mode & 134217728) == 0 && ((g_conv_mode & 268435456) != 0 || (d.C_out == 128 && m_tiles >= 2LL * cap))) {
+    const int nkb = d.R * d.S * (d.C_in / kBlockK);
+    if (!(splitk < 0 && m_tiles * (d.C_out / block_n) * 2 <= cap && nkb >= 8))
+      return convpp_forward(d, x, w, bias, residual, out, static_cast<int>(M_total), P, Q, cap, stream);
   }
 
   // --- activation map (im2col): 128-pixel boxes of 64 channels
