@@ -235,10 +235,8 @@ size_t mpx_net_input_bytes(int n, int h, int w, int c_pad);
  *   d_x [n,H,W,C_in] act16, d_w [C_out, R*S*C_in] act16, d_bias [C_out] fp32,
  *   d_residual / d_out [n,P,Q,C_out] act16 (residual may be NULL)
  *   relu: bit 0 = ReLU; bit 1 = the weights are the space-to-depth form of the 7x7 stem (4x4 taps over C_in = 64,
- *   megapose6d_b200/backbone.py: _stem_s2d; 15 of its 64 (tap, 16-channel) slices are zero by construction);
- *   bit 2 = fused 3x3/s2/p1 max-pool (models/torchvision_resnet.py:197 `self.maxpool` right after the stem's ReLU): d_out is
- *   then the ZEROED [n, (P-1)/2+1, (Q-1)/2+1, C_out] tensor and is max-reduced into; needs bit 0, no residual and
- *   block_n = 0, and returns MPX_ERR_UNSUPPORTED (nothing launched, no error text) otherwise
+ *   megapose6d_b200/backbone.py: _stem_s2d; 15 of its 64 (tap, 16-channel) slices are zero by construction); any other
+ *   bit is refused before any launch
  *   block_n: 0 = auto, else 64|128|256; max_ctas: 0 = one per SM */
 int mpx_conv2d(const void* d_x, int n, int h, int w, int c_in, const void* d_w,
                     const float* d_bias, int c_out, int r, int s, int stride, int pad_lo_h,
@@ -254,31 +252,36 @@ int mpx_conv2d_splitk(const void* d_x, int n, int h, int w, int c_in, const void
                            int pad_lo_w, int pad_hi_h, int pad_hi_w, int relu, const void* d_residual,
                            void* d_out, int block_n, int splits, void* stream);
 
-/* convolution options, default 8.  One kernel serves every shape (TMA im2col + wgmma, 128-row tiles, 64/128/256-wide
- * tiles chosen from the shape), except that C_out = 64 with at least 2 * mpx_sm_count() 256-pixel tiles (automatic tile
- * width, no K split, no pooled epilogue) runs on a pixel-major kernel: 256 pixels on the wgmma N dimension, two consumer
- * warpgroups taking alternate tiles, the epilogue staged through shared memory and stored by TMA, and the structurally
- * zero k16 steps of the space-to-depth stem (relu bit 1, c_pad 16 or 32) skipped.  The bits:
- *   8   mpx_net_forward splits the K loop of the convolutions after the stem over a thread-block cluster for batches <= 64
- *   512 launch without programmatic dependent launch
- *   262144 / 524288 cap the automatic small-batch K split (bit 3) at 2 / 1 CTAs per tile: less SM time per layer at a higher
- *       latency (set before graphs are captured; the trade for two frames in flight, frame_pipeline.py)
- *   2097152 mpx_net_forward lets the stem's epilogue max-pool (mpx_conv2d relu bit 2) instead of storing the stem output and
- *       running mpx_maxpool3x3s2 on it; the outputs are identical
- *   4194304 (bit 22) never use the pixel-major C_out = 64 kernel (the 128-row kernel serves those convolutions)
- *   8388608 (bit 23) the pixel-major kernel loads its activations by im2col (every input pixel once per filter tap) for
- *       every shape; by default a stride-1 convolution whose padded input row (W + both pads) is at most 256 pixels and
- *       whose C_in is at most 128 loads one band of whole input rows per (filter row, 64 channels) instead and reuses
- *       it over the filter's columns; the outputs are identical
- *   67108864 (bit 26) use the pixel-major C_out = 64 kernel for every convolution it can serve, whatever its size
- *   134217728 (bit 27) never use the ping-pong kernel (the 128-row kernel serves those convolutions).  By default a
- *       convolution with C_out = 128 and at least 2 * mpx_sm_count() 128-row tiles (automatic tile width, no K split, no
- *       pooled epilogue) runs on it: each of two consumer warpgroups owns a whole 128 x 128 tile, they take alternate
- *       tiles so one's epilogue overlaps the other's MMAs, and the epilogue is staged through shared memory and stored by
- *       TMA; the outputs are identical
- *   268435456 (bit 28) use the ping-pong kernel for every convolution it can serve (C_out a multiple of 128 up to 512),
- *       whatever its size
- * Other bits are accepted and have no effect. */
+/* convolution options, a sum of the MPX_CONV_* bits below; default MPX_CONV_NET_SPLITK (8).  One kernel serves every
+ * shape (TMA im2col + wgmma, 128-row tiles, 64/128/256-wide tiles chosen from the shape), except that C_out = 64 with at
+ * least 2 * mpx_sm_count() 256-pixel tiles (automatic tile width, no K split) runs on a pixel-major kernel: 256 pixels on
+ * the wgmma N dimension, two consumer warpgroups taking alternate tiles, the epilogue staged through shared memory and
+ * stored by TMA, and the structurally zero k16 steps of the space-to-depth stem (relu bit 1, c_pad 16 or 32) skipped; and
+ * that C_out = 128 with at least 2 * mpx_sm_count() 128-row tiles (automatic tile width, no K split) runs on a ping-pong
+ * kernel: each of two consumer warpgroups owns a whole 128 x 128 tile, they take alternate tiles so one's epilogue overlaps
+ * the other's MMAs, and the epilogue is staged through shared memory and stored by TMA.  The three kernels, and the
+ * pixel-major kernel's two ways of loading its activations, give identical outputs.  Other bits are accepted and have no
+ * effect. */
+/* mpx_net_forward splits the K loop of the convolutions after the stem over a thread-block cluster for batches <= 64 */
+#define MPX_CONV_NET_SPLITK 8
+/* launch without programmatic dependent launch */
+#define MPX_CONV_NO_PDL 512
+/* cap the automatic small-batch K split at 2 / 1 CTAs per tile: less SM time per layer at a higher latency (set before
+ * graphs are captured; the trade for two frames in flight, frame_pipeline.py) */
+#define MPX_CONV_SPLITK_CAP2 262144
+#define MPX_CONV_SPLITK_CAP1 524288
+/* never use the pixel-major C_out = 64 kernel (the 128-row kernel serves those convolutions) */
+#define MPX_CONV_NEVER_C64 4194304
+/* the pixel-major kernel loads its activations by im2col (every input pixel once per filter tap) for every shape; by
+ * default a stride-1 convolution whose padded input row (W + both pads) is at most 256 pixels and whose C_in is at most
+ * 128 loads one band of whole input rows per (filter row, 64 channels) instead and reuses it over the filter's columns */
+#define MPX_CONV_FORCE_IM2COL 8388608
+/* use the pixel-major C_out = 64 kernel for every convolution it can serve, whatever its size */
+#define MPX_CONV_FORCE_C64 67108864
+/* never use the ping-pong kernel (the 128-row kernel serves those convolutions) */
+#define MPX_CONV_NEVER_PP 134217728
+/* use the ping-pong kernel for every convolution it can serve (C_out a multiple of 128 up to 512), whatever its size */
+#define MPX_CONV_FORCE_PP 268435456
 int mpx_conv_set_mode(int mode);
 
 /* 3x3/s2/p1 max pool, act16 NHWC (torchvision_resnet.py:302) */

@@ -335,7 +335,8 @@ int mpx_conv2d(const void* d_x, int n, int h, int w, int c_in, const void* d_w, 
                   (reinterpret_cast<uintptr_t>(d_bias) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(d_residual) & 15) == 0,
               "mpx_conv2d: pointers must be 16-byte aligned");
-  ConvDesc d{n, h, w, c_in, c_out, r, s, stride, pad_lo_h, pad_lo_w, pad_hi_h, pad_hi_w, relu & 1, (relu >> 1) & 1, (relu >> 2) & 1};
+  MPX_REQUIRE((relu & ~3) == 0, "mpx_conv2d: relu flags 0x%x: only bits 0 and 1 are defined", relu);
+  ConvDesc d{n, h, w, c_in, c_out, r, s, stride, pad_lo_h, pad_lo_w, pad_hi_h, pad_hi_w, relu & 1, (relu >> 1) & 1};
   return conv_forward(d, d_x, d_w, d_bias, d_residual, d_out, block_n, max_ctas,
                       static_cast<cudaStream_t>(stream));
 }
@@ -356,6 +357,7 @@ int mpx_conv2d_splitk(const void* d_x, int n, int h, int w, int c_in, const void
                   (reinterpret_cast<uintptr_t>(d_out) & 15) == 0 && (reinterpret_cast<uintptr_t>(d_bias) & 15) == 0 &&
                   (reinterpret_cast<uintptr_t>(d_residual) & 15) == 0,
               "mpx_conv2d_splitk: pointers must be 16-byte aligned");
+  MPX_REQUIRE((relu & ~3) == 0, "mpx_conv2d_splitk: relu flags 0x%x: only bits 0 and 1 are defined", relu);
   ConvDesc d{n, h, w, c_in, c_out, r, s, stride, pad_lo_h, pad_lo_w, pad_hi_h, pad_hi_w, relu & 1, (relu >> 1) & 1};
   return conv_forward(d, d_x, d_w, d_bias, d_residual, d_out, block_n, 0, static_cast<cudaStream_t>(stream),
                       splits == 0 ? -1 : splits);

@@ -1,6 +1,5 @@
 // Implicit-GEMM convolution for sm_90a: TMA im2col (activations) + TMA tiled (weights) -> 128B-swizzled shared memory ->
-// wgmma (act16 x act16 -> fp32 register accumulators) -> fused epilogue (folded-BN bias, residual add, ReLU, optionally the
-// stem's 3x3/s2 max-pool) -> act16 NHWC.
+// wgmma (act16 x act16 -> fp32 register accumulators) -> fused epilogue (folded-BN bias, residual add, ReLU) -> act16 NHWC.
 //
 // Replaces the cuDNN convolutions issued by every nn.Conv2d + BatchNorm2d + ReLU (+ residual) of the
 // reference backbone (reference: src/megapose/models/torchvision_resnet.py:74-120 BasicBlock.forward,
@@ -159,18 +158,6 @@ __device__ __forceinline__ void cluster_sync_all() {
 // the 256 consumer threads only (the producer warpgroup does not take part)
 __device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
-// 3x3 / stride-2 / pad-1 max-pool epilogue: (ReLU'd, >= 0) output values are max-reduced into every pooled pixel whose
-// window contains them, four channels (two lanes' value pairs) per reduction.  The maximum is exact and order-independent
-// and the pooled tensor is zeroed before the launch, so the result equals maxpool3x3s2_kernel applied to the stored
-// convolution.
-__device__ __forceinline__ void red_max_act4(act_t* dst, uint32_t lo, uint32_t hi) {
-#ifdef MPX_ACT_BF16
-  asm volatile("red.global.max.noftz.v2.bf16x2 [%0], {%1, %2};" ::"l"(dst), "r"(lo), "r"(hi) : "memory");
-#else
-  asm volatile("red.global.max.noftz.v2.f16x2 [%0], {%1, %2};" ::"l"(dst), "r"(lo), "r"(hi) : "memory");
-#endif
-}
-
 // ---------------------------------------------------------------------------------------------
 // optional per-launch timing (bench.py roofline): CUDA events around every conv launch
 // ---------------------------------------------------------------------------------------------
@@ -222,7 +209,7 @@ int conv_profile_summary(double* total_ms, double* total_flops, long long* launc
 }
 
 // kernel-selection bits, see include/mpx.h (mpx_conv_set_mode)
-static int g_conv_mode = 8;
+static int g_conv_mode = MPX_CONV_NET_SPLITK;
 int conv_get_mode() { return g_conv_mode; }
 void conv_set_mode(int mode) { g_conv_mode = mode; }
 
@@ -237,7 +224,6 @@ struct ConvParams {
   int num_k_blocks;  // R * S * cblocks
   int m_tiles, n_tiles;
   int relu;
-  int pool;                 // 1: max-pool epilogue into `out` = the zeroed [n, (P-1)/2+1, (Q-1)/2+1, C_out] tensor
   const float* bias;        // [C_out] folded BN shift
   const act_t* residual;    // [M_total, C_out] or nullptr
   act_t* out;               // [M_total, C_out]
@@ -460,14 +446,13 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         }
         continue;
       }
-      const int pq = p.P * p.Q;
-      const int pp = (p.P - 1) / 2 + 1, pq2 = (p.Q - 1) / 2 + 1;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const long long m = m0 + row_lo + 8 * h;
         const bool valid = m < p.M_total;  // uniform over the 4 lanes of a row
         const size_t off = static_cast<size_t>(valid ? m : 0) * p.C_out + n0 + col;
-        const act_t* res_row = (valid && p.residual) ? p.residual + off : nullptr;
+        if (!valid) continue;
+        const act_t* res_row = p.residual ? p.residual + off : nullptr;
         uint32_t packed[BLOCK_N / 8];
 #pragma unroll
         for (int j = 0; j < BLOCK_N / 8; ++j) {
@@ -485,30 +470,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
           }
           packed[j] = pack_act2(f0, f1);
         }
-        if (!p.pool) {
-          if (valid) {
 #pragma unroll
-            for (int j = 0; j < BLOCK_N / 8; ++j) *reinterpret_cast<uint32_t*>(p.out + off + 8 * j) = packed[j];
-          }
-          continue;
-        }
-        uint32_t nb[BLOCK_N / 8];  // the odd lane's pair: channels col + 2, col + 3 for the even lane
-#pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) nb[j] = __shfl_xor_sync(0xffffffffu, packed[j], 1);
-        if (!valid || (lane & 1) != 0) continue;
-        const int img = static_cast<int>(m / pq);
-        const int rem = static_cast<int>(m - static_cast<long long>(img) * pq);
-        const int y = rem / p.Q, x = rem - y * p.Q;
-        // pooled rows / columns whose 3x3 window (2k-1 .. 2k+1) contains y / x
-        const int py0 = y >> 1, py1 = ((y & 1) && ((y + 1) >> 1) < pp) ? (y + 1) >> 1 : py0;
-        const int px0 = x >> 1, px1 = ((x & 1) && ((x + 1) >> 1) < pq2) ? (x + 1) >> 1 : px0;
-        for (int py = py0; py <= py1; ++py) {
-          for (int px = px0; px <= px1; ++px) {
-            act_t* dst = p.out + ((static_cast<size_t>(img) * pp + py) * pq2 + px) * p.C_out + n0 + col;
-#pragma unroll
-            for (int j = 0; j < BLOCK_N / 8; ++j) red_max_act4(dst + 8 * j, packed[j], nb[j]);
-          }
-        }
+        for (int j = 0; j < BLOCK_N / 8; ++j) *reinterpret_cast<uint32_t*>(p.out + off + 8 * j) = packed[j];
       }
     }
   }
@@ -1320,8 +1283,7 @@ static int conv64_forward(const ConvDesc& d, const void* x, const void* w, const
   p.relu = d.relu;
   p.has_residual = residual != nullptr;
   p.bias = bias;
-  // mode bit 23 keeps every shape on the im2col producer
-  const bool band = conv64_band_fits(d) && (g_conv_mode & 8388608) == 0;
+  const bool band = conv64_band_fits(d) && (g_conv_mode & MPX_CONV_FORCE_IM2COL) == 0;
   int band_n = 0;
   CUtensorMap map_x, map_w, map_res, map_out;
   int rc;
@@ -1442,8 +1404,6 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
               max_c_out);
   MPX_REQUIRE(d.stride == 1 || d.stride == 2, "conv: stride %d unsupported", d.stride);
   MPX_REQUIRE(d.R >= 1 && d.R <= 8 && d.S >= 1 && d.S <= 8, "conv: filter %dx%d unsupported", d.R, d.S);
-  // the pooled epilogue needs non-negative values (ReLU) and no residual; refused without an error text otherwise
-  if (d.pool && (!d.relu || residual != nullptr || block_n_override != 0 || splitk != 0)) return MPX_ERR_UNSUPPORTED;
   int rc = load_driver_entry_points();
   if (rc != MPX_OK) return rc;
 
@@ -1466,15 +1426,15 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
               "conv: BLOCK_N=%d invalid for C_out=%d", block_n, d.C_out);
 
   // C_out = 64 with enough 256-pixel tiles to give every CTA at least two (one per consumer warpgroup): the pixel-major
-  // kernel.  Mode bit 22 never takes it, bit 26 takes it whatever the size.  It loads its activations by filter-row band
-  // where conv64_band_fits, by im2col otherwise (or under bit 23).
+  // kernel.  MPX_CONV_NEVER_C64 never takes it, MPX_CONV_FORCE_C64 takes it whatever the size.  It loads its activations
+  // by filter-row band where conv64_band_fits, by im2col otherwise (or under MPX_CONV_FORCE_IM2COL).
   const bool aligned = (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(residual) & 15) == 0;
   const long long tiles256 = (M_total + kC64Pixels - 1) / kC64Pixels;
   const int cap = max_ctas > 0 ? max_ctas : sm_count();
-  if (d.C_out == 64 && block_n_override == 0 && splitk <= 0 && !d.pool && aligned && (g_conv_mode & 4194304) == 0 &&
-      ((g_conv_mode & 67108864) != 0 || tiles256 >= 2LL * cap)) {
+  if (d.C_out == 64 && block_n_override == 0 && splitk <= 0 && aligned && (g_conv_mode & MPX_CONV_NEVER_C64) == 0 &&
+      ((g_conv_mode & MPX_CONV_FORCE_C64) != 0 || tiles256 >= 2LL * cap)) {
     // a heuristic K split (splitk < 0) only applies below 2 * SMs / 4 128-row tiles, far under this kernel's threshold;
-    // with bit 26 a shape it would split stays on the 128-row kernel
+    // with MPX_CONV_FORCE_C64 a shape it would split stays on the 128-row kernel
     const long long m_tiles128 = (M_total + kBlockM - 1) / kBlockM;
     const int nkb = d.R * d.S * (d.C_in / kBlockK);
     if (!(splitk < 0 && m_tiles128 * 2 <= cap && nkb >= 8))
@@ -1484,11 +1444,12 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
   // C_out = 128 with at least two 128 x 128 tiles per CTA: the ping-pong kernel.  C_out = 256 and 512 keep the 128 x 256
   // tiles of the 128-row kernel by default: a 128-wide tile fills 32 KB of shared memory per 128 x 128 x 64 block where
   // those fill 48 KB per twice the work, and on an H100 that costs the 3x3 convolutions of layers 3 and 4 more than the
-  // overlapped epilogue gains (DESIGN 3.1).  Mode bit 27 never takes it, bit 28 takes it for every C_out it serves
-  // (multiples of 128 up to 512), whatever the size, except for a shape the small-batch heuristic splits over K.
+  // overlapped epilogue gains (DESIGN 3.1).  MPX_CONV_NEVER_PP never takes it, MPX_CONV_FORCE_PP takes it for every C_out
+  // it serves (multiples of 128 up to 512), whatever the size, except for a shape the small-batch heuristic splits over K.
   const long long m_tiles = (M_total + kBlockM - 1) / kBlockM;
-  if (d.C_out % 128 == 0 && d.C_out <= 512 && block_n_override == 0 && splitk <= 0 && !d.pool && aligned &&
-      (g_conv_mode & 134217728) == 0 && ((g_conv_mode & 268435456) != 0 || (d.C_out == 128 && m_tiles >= 2LL * cap))) {
+  if (d.C_out % 128 == 0 && d.C_out <= 512 && block_n_override == 0 && splitk <= 0 && aligned &&
+      (g_conv_mode & MPX_CONV_NEVER_PP) == 0 &&
+      ((g_conv_mode & MPX_CONV_FORCE_PP) != 0 || (d.C_out == 128 && m_tiles >= 2LL * cap))) {
     const int nkb = d.R * d.S * (d.C_in / kBlockK);
     if (!(splitk < 0 && m_tiles * (d.C_out / block_n) * 2 <= cap && nkb >= 8))
       return convpp_forward(d, x, w, bias, residual, out, static_cast<int>(M_total), P, Q, cap, stream);
@@ -1516,7 +1477,6 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
   p.m_tiles = static_cast<int>((M_total + kBlockM - 1) / kBlockM);
   p.n_tiles = d.C_out / block_n;
   p.relu = d.relu;
-  p.pool = d.pool;
   p.bias = bias;
   p.residual = reinterpret_cast<const act_t*>(residual);
   p.out = reinterpret_cast<act_t*>(out);
@@ -1530,9 +1490,11 @@ int conv_forward(const ConvDesc& d, const void* x, const void* w, const float* b
       want = p.num_k_blocks / 4;
       if (want > sms / tiles) want = sms / tiles;
     }
-    // bits 18 / 19 of the mode cap the automatic split at 2 / 1: fewer, longer CTAs -- less SM time per layer at a higher
-    // latency, the better trade when another frame's kernels fill the device beside this one (frame_pipeline.py)
-    const int cap = (splitk < 0 && (g_conv_mode & 524288)) ? 1 : ((splitk < 0 && (g_conv_mode & 262144)) ? 2 : 8);
+    // MPX_CONV_SPLITK_CAP2 / _CAP1 cap the automatic split at 2 / 1: fewer, longer CTAs -- less SM time per layer at a
+    // higher latency, the better trade when another frame's kernels fill the device beside this one (frame_pipeline.py)
+    const int cap = (splitk < 0 && (g_conv_mode & MPX_CONV_SPLITK_CAP1))
+                        ? 1
+                        : ((splitk < 0 && (g_conv_mode & MPX_CONV_SPLITK_CAP2)) ? 2 : 8);
     int splits = 1;
     while (splits * 2 <= want && splits * 2 <= cap && splits * 2 <= p.num_k_blocks) splits *= 2;
     p.splits = splits;

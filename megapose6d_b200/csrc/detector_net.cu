@@ -239,11 +239,11 @@ static int fpn_forward_direct(const Fpn* f, const float* images, int n, int h, i
   auto buf = [&](int b) -> void* { return base + off[b]; };
   const FpnDims dims = fpn_dims(h, w);
   // small batches: the deep convolutions split their K loop over a cluster, as in mpx_net_forward
-  const int sk = ((conv_get_mode() & 8) != 0 && n <= 64) ? -1 : 0;
+  const int sk = ((conv_get_mode() & MPX_CONV_NET_SPLITK) != 0 && n <= 64) ? -1 : 0;
   auto conv = [&](int wi, int H, int W, int c_in, int c_out, int k, int stride, int relu, const void* x,
                   const void* residual, void* out) {
     const int pad = k / 2;
-    ConvDesc d{n, H, W, c_in, c_out, k, k, stride, pad, pad, pad, pad, relu, 0, 0};
+    ConvDesc d{n, H, W, c_in, c_out, k, k, stride, pad, pad, pad, pad, relu, 0};
     return conv_forward(d, x, f->conv_w[wi], f->conv_b[wi], residual, out, 0, 0, stream, sk, 2048);
   };
   int rc;
@@ -252,7 +252,7 @@ static int fpn_forward_direct(const Fpn* f, const float* images, int n, int h, i
   ++g_launches;
   {
     // 7x7/s2/p3 stem as the 4x4/s1 convolution (pad 2 low, 1 high) over the space-to-depth input, then ReLU, max-pool
-    ConvDesc d{n, h / 2, w / 2, 64, 64, 4, 4, 1, 2, 2, 1, 1, 1, 1, 0};
+    ConvDesc d{n, h / 2, w / 2, 64, 64, 4, 4, 1, 2, 2, 1, 1, 1, 1};
     rc = conv_forward(d, buf(kBufX), f->conv_w[0], f->conv_b[0], nullptr, buf(kBufStem), 0, 0, stream, 0, 2048);
     if (rc != MPX_OK) return rc;
     rc = maxpool3x3s2(buf(kBufStem), n, h / 2, w / 2, 64, buf(kBufPool0), stream);

@@ -7,6 +7,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include "../../include/mpx.h"
+
 namespace mpx {
 
 // ---------------------------------------------------------------------------------------------
@@ -130,7 +132,7 @@ __device__ __forceinline__ float depth_norm(float d, float z, int kind) {
 // before it touches memory the predecessor writes (or writes memory the predecessor reads); everything before that --
 // barrier set-up, descriptor prefetch, constant loads -- overlaps with the predecessor's tail.  The chains of
 // small-batch kernels (36 convolutions of ~6-10 us each per network forward) are bound by exactly that fixed cost.
-// Without a PDL-aware predecessor both calls are no-ops.  mpx_conv_set_mode bit 9 (512) launches without the attribute.
+// Without a PDL-aware predecessor both calls are no-ops.  Mode bit MPX_CONV_NO_PDL launches without the attribute.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -152,7 +154,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     attr[n].val.clusterDim.z = 1;
     ++n;
   }
-  if ((conv_get_mode() & 512) == 0) {
+  if ((conv_get_mode() & MPX_CONV_NO_PDL) == 0) {
     attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[n].val.programmaticStreamSerializationAllowed = 1;
     ++n;
@@ -179,9 +181,6 @@ struct ConvDesc {
   int pad_lo_h, pad_lo_w, pad_hi_h, pad_hi_w;
   int relu;
   int s2d_stem;  // 1: the weights are the space-to-depth form of the 7x7 stem (megapose6d_b200/backbone.py: _stem_s2d)
-  int pool;      // 1: `out` is the ZERO-INITIALISED [n, (H-1)/2+1, (W-1)/2+1, C_out] tensor and receives the 3x3/s2/p1 max-pool of
-                 //    the (ReLU'd) result through vector max-reductions; conv_forward returns MPX_ERR_UNSUPPORTED (no error set)
-                 //    when no kernel with that epilogue serves the shape
 };
 // splitk: 0 = never, -1 = heuristic (few output tiles, long K loop), 1|2|4|8 = that many k-splits (cluster size)
 // max_c_out: the largest C_out the caller accepts (512 for the single-convolution entry points and the pose networks,

@@ -351,20 +351,9 @@ int net_forward(const Net* cnet, const void* x, int n, int h, int w, float* out,
   return MPX_OK;
 }
 
-// Stem convolution + ReLU followed by the 3x3/s2/p1 max-pool.  With mode bit 21 (2097152) the convolution pools in its
-// epilogue (max-reductions into the zeroed pooled tensor): the full-resolution stem output -- 2.46 MB per sample at 240x320,
-// written once and read once by nothing but the pool -- never exists.  Falls back to the two kernels when the shape is not
-// served (the memset is then wasted, nothing else).
-static int stem_and_pool(ConvDesc d, const void* x, const void* w, const float* b, void* buf_stem, void* buf_pool,
+// Stem convolution + ReLU into buf_stem, then the 3x3/s2/p1 max-pool into buf_pool.
+static int stem_and_pool(const ConvDesc& d, const void* x, const void* w, const float* b, void* buf_stem, void* buf_pool,
                          cudaStream_t stream) {
-  const int hp = (d.H + 2 - 3) / 2 + 1, wp = (d.W + 2 - 3) / 2 + 1;
-  if ((conv_get_mode() & 2097152) != 0 && d.relu) {
-    MPX_CHECK_CUDA(cudaMemsetAsync(buf_pool, 0, static_cast<size_t>(d.n_img) * hp * wp * d.C_out * 2, stream));
-    d.pool = 1;
-    const int rc = conv_forward(d, x, w, b, nullptr, buf_pool, 0, 0, stream);
-    if (rc != MPX_ERR_UNSUPPORTED) return rc;
-    d.pool = 0;
-  }
   const int rc = conv_forward(d, x, w, b, nullptr, buf_stem, 0, 0, stream);
   if (rc != MPX_OK) return rc;
   return maxpool3x3s2(buf_stem, d.n_img, d.H, d.W, d.C_out, buf_pool, stream);
@@ -385,7 +374,7 @@ static int net_forward_preact(const Net* net, const void* x, int n, int h, int w
   void* buf_stem = base;
   void* bufs[5];
   for (int i = 0; i < 5; ++i) bufs[i] = base + stem_bytes + i * l1_bytes;
-  const int sk = ((conv_get_mode() & 8) != 0 && n <= 64) ? -1 : 0;
+  const int sk = ((conv_get_mode() & MPX_CONV_NET_SPLITK) != 0 && n <= 64) ? -1 : 0;
   int rc;
   {
     ConvDesc d{n, hs, ws, 4 * net->c_pad, 64, 3, 3, 1, 1, 1, 1, 1, 1, 0};
@@ -489,7 +478,7 @@ static int net_forward_direct(const Net* net, const void* x, int n, int h, int w
   void* buf_stem = base;
   void* bufs[3] = {base + stem_bytes, base + stem_bytes + l1_bytes, base + stem_bytes + 2 * l1_bytes};
   // small batches (refiner iterations, final scoring): layers 2-4 split their K loop over a cluster
-  const int sk = ((conv_get_mode() & 8) != 0 && n <= 64) ? -1 : 0;
+  const int sk = ((conv_get_mode() & MPX_CONV_NET_SPLITK) != 0 && n <= 64) ? -1 : 0;
 
   if (net->preact) return net_forward_preact(net, x, n, h, w, out, workspace, stream);
   int ci = 0;

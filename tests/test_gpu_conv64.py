@@ -14,20 +14,18 @@ import pytest
 import torch
 
 from megapose6d_b200 import _abi
-from tests.test_gpu_conv_exact import (ACT, P0, P1, SMS_H100, STEM, TINY, UNIT, Conv, _conv64, _gen, _guarded,
-                                       _guards_intact, _launch, _out_dim, _problem, _to_act)
+from tests.test_gpu_conv_exact import (ACT, DEFAULT_CONV_MODE, FORCE_C64, NEVER_C64, P0, P1, SMS_H100, STEM, TINY, UNIT,
+                                       Conv, _conv64, _gen, _guarded, _guards_intact, _launch, _out_dim, _problem, _to_act,
+                                       device_kernels, mode_fixture)
 
 gpu = pytest.mark.gpu
-DEFAULT_CONV_MODE = 8
-NEVER_C64 = 4194304  # mode bit 22: never the pixel-major kernel
-FORCE_C64 = 67108864  # mode bit 26: the pixel-major kernel for every convolution it can serve
 C64_PIXELS = 256
 C64_STAGES = 4
 
 
 def _uses_conv64(c: Conv, mode: int, sms: int, out_aligned: bool = True) -> bool:
     """conv_forward's choice of conv64_wgmma_kernel for mpx_conv2d (no K split)."""
-    if c.cout != 64 or c.block_n != 0 or c.splits is not None or c.pool or not out_aligned or mode & NEVER_C64:
+    if c.cout != 64 or c.block_n != 0 or c.splits is not None or not out_aligned or mode & NEVER_C64:
         return False
     P, Q = _out_dim(c.h, c.pads[0], c.pads[2], c.r, c.stride), _out_dim(c.w, c.pads[1], c.pads[3], c.s, c.stride)
     tiles = -(-c.n * P * Q // C64_PIXELS)
@@ -72,27 +70,7 @@ CASES = [
 assert len({c.name for c in CASES}) == len(CASES)
 
 
-def _set_mode(mode):
-    _abi.lib().mpx_conv_set_mode(mode)
-
-
-@pytest.fixture
-def forced():
-    _set_mode(FORCE_C64 | DEFAULT_CONV_MODE)
-    yield
-    _set_mode(DEFAULT_CONV_MODE)
-
-
-def _device_kernels(fn):
-    """Runs `fn` under torch.profiler (CUDA activities) and returns its result and the names of the kernels it launched:
-    the proof that a case ran on the kernel it is meant for, since both kernels give the same bits."""
-    from torch.profiler import ProfilerActivity, profile
-
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        out = fn()
-        torch.cuda.synchronize()
-    names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-    return out, names
+forced = mode_fixture(FORCE_C64 | DEFAULT_CONV_MODE)
 
 
 def _ran_conv64(names):
@@ -105,7 +83,7 @@ def test_conv64_bit_exact(case, forced):
     if case.family == "saturate" and ACT != torch.float16:
         pytest.skip("saturation at +-65504 is the fp16 conversion")
     x, w, b, r, want = _problem(case, _gen(case.name))
-    got, names = _device_kernels(lambda: _launch(case, x, w, b, r))
+    got, names = device_kernels(lambda: _launch(case, x, w, b, r), "conv64_wgmma_kernel")
     assert _ran_conv64(names) and not any("conv_wgmma_kernel" in n for n in names), names
     bad = got.float() != want.float()
     assert not bad.any(), f"{int(bad.sum())} of {bad.numel()} outputs differ, first at {bad.nonzero()[0].tolist()}"
@@ -178,9 +156,9 @@ def test_stem_skips_structural_zero_slices(cin, forced):
     want_clean = _to_act(torch.relu(_conv64(x, w_clean, 1, STEM) + b))
     want_garbage = _to_act(torch.relu(_conv64(x, w_clean + garbage, 1, STEM) + b))
     assert not torch.equal(want_clean, want_garbage)
-    got, names = _device_kernels(lambda: _run(c, x, w_clean + garbage, b, None, flags=1 | 2))
+    got, names = device_kernels(lambda: _run(c, x, w_clean + garbage, b, None, flags=1 | 2), "conv64_wgmma_kernel")
     assert _ran_conv64(names) and torch.equal(got, want_clean)
-    got, names = _device_kernels(lambda: _run(c, x, w_clean + garbage, b, None, flags=1))
+    got, names = device_kernels(lambda: _run(c, x, w_clean + garbage, b, None, flags=1), "conv64_wgmma_kernel")
     assert _ran_conv64(names) and torch.equal(got, want_garbage)
 
 
@@ -207,7 +185,7 @@ def test_conv64_gaussian_data_within_rounding_bound(case):
     if case.relu:
         y64 = torch.relu(y64)
     mag = _conv64(x.abs(), w.abs(), case.stride, case.pads) + b.abs() + (r.abs() if r is not None else 0)
-    got, names = _device_kernels(lambda: _run(case, x, w, b, r, flags=int(case.relu)))
+    got, names = device_kernels(lambda: _run(case, x, w, b, r, flags=int(case.relu)), "conv64_wgmma_kernel")
     assert _ran_conv64(names), names
     got = got.double()
     err = (got - y64).abs()
@@ -234,9 +212,9 @@ def test_network_forward_with_and_without_conv64():
     try:
         lib.mpx_net_set_graphs(0)
         lib.mpx_conv_set_mode(DEFAULT_CONV_MODE | NEVER_C64)
-        old, names_old = _device_kernels(lambda: eng.forward(x, 240, 320).clone())
+        old, names_old = device_kernels(lambda: eng.forward(x, 240, 320).clone())
         lib.mpx_conv_set_mode(DEFAULT_CONV_MODE)
-        new, names_new = _device_kernels(lambda: eng.forward(x, 240, 320).clone())
+        new, names_new = device_kernels(lambda: eng.forward(x, 240, 320).clone(), "conv64_wgmma_kernel", 7)
     finally:
         lib.mpx_net_set_graphs(1)
         lib.mpx_conv_set_mode(DEFAULT_CONV_MODE)
@@ -298,6 +276,6 @@ def test_dispatch_rule_covers_the_cases():
     assert _uses_conv64(dataclasses.replace(layer1, n=576), DEFAULT_CONV_MODE, SMS_H100)
     assert not _uses_conv64(dataclasses.replace(layer1, n=576), DEFAULT_CONV_MODE | NEVER_C64, SMS_H100)
     assert not _uses_conv64(dataclasses.replace(layer1, n=576), FORCE_C64 | NEVER_C64, SMS_H100)
-    for other in (dict(cout=128), dict(block_n=64), dict(splits=1), dict(pool=True)):
+    for other in (dict(cout=128), dict(block_n=64), dict(splits=1)):
         assert not _uses_conv64(dataclasses.replace(layer1, n=576, **other), FORCE_C64, SMS_H100), other
     assert not _uses_conv64(dataclasses.replace(layer1, n=576), FORCE_C64, SMS_H100, out_aligned=False)

@@ -18,13 +18,12 @@ import pytest
 import torch
 
 from megapose6d_b200 import _abi
-from tests.test_gpu_conv64 import (C64_PIXELS, DEFAULT_CONV_MODE, FORCE_C64, NEVER_C64, _c64, _device_kernels,
-                                   _stem_zero_slices, _uses_conv64)
-from tests.test_gpu_conv_exact import (ACT, P1, SMS_H100, STEM, Conv, _conv64, _gen, _guarded, _guards_intact, _launch,
-                                       _out_dim, _problem, _to_act)
+from tests.test_gpu_conv64 import C64_PIXELS, _c64, _stem_zero_slices, _uses_conv64
+from tests.test_gpu_conv_exact import (ACT, DEFAULT_CONV_MODE, FORCE_C64, FORCE_IM2COL, NEVER_C64, P1, SMS_H100, STEM, Conv,
+                                       _conv64, _gen, _guarded, _guards_intact, _launch, _out_dim, _problem, _to_act,
+                                       device_kernels, mode_fixture, set_mode)
 
 gpu = pytest.mark.gpu
-FORCE_IM2COL = 8388608  # mode bit 23: the pixel-major kernel loads by im2col for every shape
 BAND_SLOTS = 3
 LAYOUT_BYTES = 227 * 1024 - 1536  # shared memory less alignment slack, barriers and bias
 
@@ -60,25 +59,7 @@ def _conv64_instances(names):
     return out
 
 
-def _kernels(fn, launches=1):
-    """_device_kernels, repeated (at most three captures) until the capture holds the `launches` conv64_wgmma_kernel
-    launches that fn makes: torch.profiler can drop device activity from one of many short captures, while a launch it
-    does record always names the instantiation that ran."""
-    for _ in range(3):
-        out, names = _device_kernels(fn)
-        if len(_conv64_instances(names)) >= launches:
-            break
-    return out, names
-
-
-def _set_mode(mode):
-    _abi.lib().mpx_conv_set_mode(mode)
-
-
-@pytest.fixture
-def restore_mode():
-    yield
-    _set_mode(DEFAULT_CONV_MODE)
+restore_mode = mode_fixture()
 
 
 # geometry of the coarse network at the two render sizes: stem over the space-to-depth input, layer1 after the max-pool
@@ -131,13 +112,13 @@ def test_band_bit_exact(case, restore_mode):
     plan = _band_plan(case)
     assert plan is not None
     x, w, b, r, want = _problem(case, _gen(case.name))
-    _set_mode(DEFAULT_CONV_MODE | FORCE_C64)
-    got, names = _kernels(lambda: _launch(case, x, w, b, r))
+    set_mode(DEFAULT_CONV_MODE | FORCE_C64)
+    got, names = device_kernels(lambda: _launch(case, x, w, b, r), "conv64_wgmma_kernel")
     assert _conv64_instances(names) == [(0, plan.n)], names
     bad = got.float() != want.float()
     assert not bad.any(), f"{int(bad.sum())} of {bad.numel()} outputs differ, first at {bad.nonzero()[0].tolist()}"
-    _set_mode(DEFAULT_CONV_MODE | FORCE_C64 | FORCE_IM2COL)
-    old, names = _kernels(lambda: _launch(case, x, w, b, r))
+    set_mode(DEFAULT_CONV_MODE | FORCE_C64 | FORCE_IM2COL)
+    old, names = device_kernels(lambda: _launch(case, x, w, b, r), "conv64_wgmma_kernel")
     assert _conv64_instances(names) == [(0, 0)], names
     assert torch.equal(old, got)
 
@@ -174,12 +155,12 @@ def test_band_stem_skips_structural_zero_slices(cin, size, restore_mode):
     garbage = torch.where(zero, torch.randint(1, 4, w.shape, generator=g, device=w.device).double(), torch.zeros_like(w))
     want = _to_act(torch.relu(_conv64(x, w_clean, 1, STEM) + b))
     assert not torch.equal(want, _to_act(torch.relu(_conv64(x, w_clean + garbage, 1, STEM) + b)))
-    _set_mode(DEFAULT_CONV_MODE | FORCE_C64)
-    got, names = _kernels(lambda: _run_stem(c, x, w_clean + garbage, b))
+    set_mode(DEFAULT_CONV_MODE | FORCE_C64)
+    got, names = device_kernels(lambda: _run_stem(c, x, w_clean + garbage, b), "conv64_wgmma_kernel")
     assert _conv64_instances(names) == [(cin // 64, _band_plan(c).n)], names
     assert torch.equal(got, want)
-    _set_mode(DEFAULT_CONV_MODE | FORCE_C64 | FORCE_IM2COL)
-    old, names = _kernels(lambda: _run_stem(c, x, w_clean + garbage, b))
+    set_mode(DEFAULT_CONV_MODE | FORCE_C64 | FORCE_IM2COL)
+    old, names = device_kernels(lambda: _run_stem(c, x, w_clean + garbage, b), "conv64_wgmma_kernel")
     assert _conv64_instances(names) == [(cin // 64, 0)], names
     assert torch.equal(old, got)
 
@@ -202,12 +183,12 @@ def test_network_forward_band_and_im2col_identical(size, n, restore_mode):
     lib = _abi.lib()
     try:
         lib.mpx_net_set_graphs(0)
-        _set_mode(DEFAULT_CONV_MODE)
+        set_mode(DEFAULT_CONV_MODE)
         eng.forward(x, h, w)  # workspace and first launches outside the profiled window
         torch.cuda.synchronize()
-        new, names_new = _kernels(lambda: eng.forward(x, h, w).clone(), 7)
-        _set_mode(DEFAULT_CONV_MODE | FORCE_IM2COL)
-        old, names_old = _kernels(lambda: eng.forward(x, h, w).clone(), 7)
+        new, names_new = device_kernels(lambda: eng.forward(x, h, w).clone(), "conv64_wgmma_kernel", 7)
+        set_mode(DEFAULT_CONV_MODE | FORCE_IM2COL)
+        old, names_old = device_kernels(lambda: eng.forward(x, h, w).clone(), "conv64_wgmma_kernel", 7)
     finally:
         lib.mpx_net_set_graphs(1)
     inst_new, inst_old = _conv64_instances(names_new), _conv64_instances(names_old)

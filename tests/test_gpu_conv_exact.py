@@ -15,6 +15,8 @@ The generator asserts its own precondition on the host (conv(|x|, |w|) + |b| + |
 
 _plan restates the host-side choices of conv_forward / launch_conv (tile width, ring depth, grid, tiles per CTA, K split,
 images per tile, driver fix-up); test_plan_covers_every_decision_point (no GPU) checks that CASES reaches each of them.
+
+The mpx_conv_set_mode bits, set_mode, mode_fixture and device_kernels are defined here for every convolution test.
 """
 from __future__ import annotations
 
@@ -39,8 +41,6 @@ TINY = 2.0 ** -25 if ACT == torch.float16 else 2.0 ** -134  # half the smallest 
 STAGES = {64: 8, 128: 6, 256: 4}  # ConvCfg<BLOCK_N>::kStages
 BLOCK_M = 128
 SMS_H100 = 132
-DEFAULT_CONV_MODE = 8
-NO_PDL = 512  # mode bit 9: launch without programmatic dependent launch
 P0, P1, STEM = (0, 0, 0, 0), (1, 1, 1, 1), (2, 2, 1, 1)
 
 
@@ -61,8 +61,52 @@ class Conv:
     block_n: int = 0  # 0: automatic
     max_ctas: int = 0  # 0: one CTA per SM
     splits: Optional[int] = None  # None: mpx_conv2d; else mpx_conv2d_splitk with this split count (0: heuristic)
-    pool: bool = False  # relu bit 2: the 3x3 / s2 / p1 max-pool epilogue
     family: str = "exact"  # exact | ties | saturate
+
+
+# ---------------------------------------------------------------------------------------------
+# kernel selection: the mpx_conv_set_mode bits of include/mpx.h (MPX_CONV_*)
+# ---------------------------------------------------------------------------------------------
+DEFAULT_CONV_MODE = 8  # MPX_CONV_NET_SPLITK, the library's default
+NO_PDL = 512  # MPX_CONV_NO_PDL: launch without programmatic dependent launch
+NEVER_C64 = 4194304  # MPX_CONV_NEVER_C64: never the pixel-major C_out = 64 kernel
+FORCE_IM2COL = 8388608  # MPX_CONV_FORCE_IM2COL: the pixel-major kernel loads by im2col for every shape
+FORCE_C64 = 67108864  # MPX_CONV_FORCE_C64: the pixel-major kernel for every convolution it can serve
+NEVER_PP = 134217728  # MPX_CONV_NEVER_PP: never the ping-pong kernel
+FORCE_PP = 268435456  # MPX_CONV_FORCE_PP: the ping-pong kernel for every convolution it can serve
+
+
+def set_mode(mode):
+    _abi.lib().mpx_conv_set_mode(mode)
+
+
+def mode_fixture(mode=None):
+    """A fixture that sets `mode` (when given) for the test and restores DEFAULT_CONV_MODE after it."""
+    @pytest.fixture
+    def fixture():
+        if mode is not None:
+            set_mode(mode)
+        yield
+        set_mode(DEFAULT_CONV_MODE)
+    return fixture
+
+
+def device_kernels(fn, kernel=None, launches=1):
+    """Runs `fn` under torch.profiler (CUDA activities) and returns its result and the names of the kernels it launched:
+    the proof that a case ran on the kernel it is meant for, since every kernel gives the same bits.  With `kernel`, `fn`
+    is captured again (at most three captures) until the capture holds `launches` launches whose name contains it:
+    torch.profiler can drop device activity from one of many short captures, while a launch it does record always names
+    the kernel that ran."""
+    from torch.profiler import ProfilerActivity, profile
+
+    for _ in range(3 if kernel else 1):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            out = fn()
+            torch.cuda.synchronize()
+        names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
+        if kernel is None or sum(kernel in n for n in names) >= launches:
+            break
+    return out, names
 
 
 # ---------------------------------------------------------------------------------------------
@@ -197,13 +241,6 @@ CASES = _ring_cases() + [
     Conv("splitk_two_mtiles", 2, 10, 10, 128, 256, 3, 3, pads=P1, relu=True, res=True, block_n=128, splits=4),
     Conv("splitk_s2", 1, 30, 40, 128, 256, 3, 3, stride=2, pads=P1, relu=True, block_n=64, splits=4),
 ] + _splitk_epilogue_cases() + [
-    # pooled epilogue (ReLU + 3x3/s2/p1 max-pool into the zeroed pooled tensor)
-    Conv("pool_p_odd_q_odd_ctas1", 2, 17, 23, 64, 64, 3, 3, pads=P1, relu=True, pool=True, max_ctas=1),
-    Conv("pool_p_even_q_even_ctas2", 2, 16, 22, 64, 64, 3, 3, pads=P1, relu=True, pool=True, max_ctas=2),
-    Conv("pool_p_odd_q_even", 3, 17, 22, 64, 64, 3, 3, pads=P1, relu=True, pool=True),
-    Conv("pool_p_even_q_odd_ctas2", 3, 16, 23, 64, 64, 3, 3, pads=P1, relu=True, pool=True, max_ctas=2),
-    Conv("pool_stem_4x4", 2, 24, 32, 64, 64, 4, 4, pads=STEM, relu=True, pool=True),
-    Conv("pool_c128_ctas1", 1, 13, 11, 64, 128, 3, 3, pads=P1, relu=True, pool=True, max_ctas=1),
     # rounding: round-to-nearest-even ties, and saturation at the largest finite value
     Conv("ties_direct", 2, 9, 11, 64, 128, 3, 3, pads=P1, family="ties"),
     Conv("ties_direct_relu_res", 2, 9, 11, 64, 256, 3, 3, pads=P1, relu=True, res=True, family="ties"),
@@ -281,8 +318,6 @@ def _problem(c: Conv, gen):
         y = y + r
     if c.relu:
         y = torch.relu(y)
-    if c.pool:
-        y = F.max_pool2d(y.permute(0, 3, 1, 2), 3, 2, 1).permute(0, 2, 3, 1)
     return x, w, b, r, _to_act(y)
 
 
@@ -301,7 +336,7 @@ def _guards_intact(buf, guard, fill):
 
 def _run_conv(c: Conv, x, w, b, r, out, lib):
     args = (_abi.ptr(x), c.n, c.h, c.w, c.cin, _abi.ptr(w), _abi.ptr(b), c.cout, c.r, c.s, c.stride, *c.pads,
-            int(c.relu) | (4 if c.pool else 0), _abi.ptr(r), _abi.ptr(out))
+            int(c.relu), _abi.ptr(r), _abi.ptr(out))
     if c.splits is None:
         return lib.mpx_conv2d(*args, c.block_n, c.max_ctas, _abi.stream_ptr())
     return lib.mpx_conv2d_splitk(*args, c.block_n, c.splits, _abi.stream_ptr())
@@ -320,11 +355,8 @@ def _launch(c: Conv, x, w, b, r):
         rv.copy_(r)
     wv = w.reshape(c.cout, -1).to(ACT).contiguous()
     bv = b.float().contiguous()
-    shape = (c.n, (plan.P - 1) // 2 + 1, (plan.Q - 1) // 2 + 1, c.cout) if c.pool else (c.n, plan.P, plan.Q, c.cout)
     guard = BLOCK_M * c.cout
-    obuf, out = _guarded(shape, guard, float("nan"))
-    if c.pool:
-        out.zero_()
+    obuf, out = _guarded((c.n, plan.P, plan.Q, c.cout), guard, float("nan"))
     launches = lib.mpx_launch_count()
     _abi.check(_run_conv(c, xv, wv, bv, rv, out, lib))
     torch.cuda.synchronize()
@@ -401,7 +433,7 @@ def test_dependent_chain_on_one_stream(mode):
     torch.cuda.synchronize()
     s = _abi.stream_ptr()
     try:
-        lib.mpx_conv_set_mode(mode)
+        set_mode(mode)
         _abi.check(lib.mpx_conv2d(_abi.ptr(xv), n, h, w, 64, _abi.ptr(ws[0]), _abi.ptr(bs[0]), 64, 3, 3, 1, *P1, 1, None,
                                   _abi.ptr(a1), 0, 0, s))
         _abi.check(lib.mpx_conv2d(_abi.ptr(a1), n, h, w, 64, _abi.ptr(ws[1]), _abi.ptr(bs[1]), 64, 3, 3, 1, *P1, 1,
@@ -410,7 +442,7 @@ def test_dependent_chain_on_one_stream(mode):
                                   _abi.ptr(a3), 0, 0, s))
         torch.cuda.synchronize()
     finally:
-        lib.mpx_conv_set_mode(DEFAULT_CONV_MODE)
+        set_mode(DEFAULT_CONV_MODE)
     for got, want in ((a1, y1), (a2, y2), (a3, y3)):
         assert torch.equal(got, _to_act(want))
 
@@ -437,11 +469,14 @@ def _contract_cases():
         ("splitk_block_n_0", dict(splitk=True, block_n=0, extra=2), "block_n must be 64|128|256"),
         ("splitk_cin_48", dict(splitk=True, block_n=64, extra=2, cin=48), "C_in=48 must be a multiple of 64"),
         ("splitk_block_n_256_cout_192", dict(splitk=True, cout=192, block_n=256, extra=2), "BLOCK_N=256 invalid"),
-        # pooled epilogue without its preconditions: MPX_ERR_UNSUPPORTED, no error text
-        ("pool_with_residual", dict(relu=5, res=True), None),
-        ("pool_with_block_n", dict(relu=5, block_n=64), None),
-        ("pool_without_relu", dict(relu=4), None),
     ]
+    for relu in (4, 5, 8):  # relu flags: bits 0 (ReLU) and 1 (space-to-depth stem weights) only
+        cases.append((f"relu_flags_{relu}", dict(relu=relu), f"relu flags 0x{relu:x}: only bits 0 and 1 are defined"))
+        cases.append((f"splitk_relu_flags_{relu}", dict(splitk=True, block_n=64, extra=2, relu=relu),
+                      f"relu flags 0x{relu:x}: only bits 0 and 1 are defined"))
+    # bit 2 beside a residual or an explicit tile width: refused by the flag check before anything else
+    cases.append(("relu_flags_5_with_residual", dict(relu=5, res=True), "relu flags 0x5: only bits 0 and 1 are defined"))
+    cases.append(("relu_flags_5_with_block_n_64", dict(relu=5, block_n=64), "relu flags 0x5: only bits 0 and 1 are defined"))
     return [(name, {**ok, **kw}, msg) for name, kw, msg in cases]
 
 
@@ -451,7 +486,7 @@ CONTRACT_CASES = _contract_cases()
 @gpu
 @pytest.mark.parametrize("name,a,msg", CONTRACT_CASES, ids=[c[0] for c in CONTRACT_CASES])
 def test_conv_refuses_unsupported_arguments(name, a, msg):
-    """Every refusal returns non-zero with its message (or MPX_ERR_UNSUPPORTED without one) and launches nothing."""
+    """Every refusal returns non-zero with its message and launches nothing."""
     lib = _abi.lib()
     x = torch.zeros(1 << 16, device="cuda", dtype=ACT)
     w = torch.zeros(1 << 20, device="cuda", dtype=ACT)
@@ -459,10 +494,9 @@ def test_conv_refuses_unsupported_arguments(name, a, msg):
     res = torch.zeros(1 << 16, device="cuda", dtype=ACT) if a["res"] else None
     out = torch.zeros(1 << 16, device="cuda", dtype=ACT)
     torch.cuda.synchronize()
-    # a known message first, so that a refusal without text is visible as an unchanged message
+    # a known message first, so that a message left by an earlier call cannot pass for this refusal's
     assert lib.mpx_conv2d(_abi.ptr(x), 1, 8, 8, 32, _abi.ptr(w), _abi.ptr(b), 64, 1, 1, 1, *P0, 0, None, _abi.ptr(out),
                           0, 0, _abi.stream_ptr()) == -1
-    before_msg = lib.mpx_last_error()
     launches = lib.mpx_launch_count()
     fn = lib.mpx_conv2d_splitk if a["splitk"] else lib.mpx_conv2d
     rc = fn(_abi.ptr(x) + a["misalign"], a["n"], a["h"], a["w"], a["cin"], _abi.ptr(w), _abi.ptr(b), a["cout"], a["r"],
@@ -470,10 +504,7 @@ def test_conv_refuses_unsupported_arguments(name, a, msg):
             a["extra"] if a["splitk"] else 0, _abi.stream_ptr())
     torch.cuda.synchronize()
     assert lib.mpx_launch_count() == launches
-    if msg is None:
-        assert rc == -3 and lib.mpx_last_error() == before_msg
-    else:
-        assert rc == -1 and msg.encode() in lib.mpx_last_error(), (rc, lib.mpx_last_error())
+    assert rc == -1 and msg.encode() in lib.mpx_last_error(), (rc, lib.mpx_last_error())
 
 
 GAUSS_CASES = [
@@ -580,12 +611,6 @@ def test_plan_covers_every_decision_point():
                 need[f"split at BLOCK_N {bn}, relu {relu}, residual {res}"] = (
                     lambda c, p, bn=bn, relu=relu, res=res: p.splits > 1 and p.block_n == bn and c.relu == relu and
                     c.res == res)
-    for pp in (0, 1):
-        for qq in (0, 1):
-            need[f"pooled, P % 2 == {pp}, Q % 2 == {qq}"] = \
-                lambda c, p, pp=pp, qq=qq: c.pool and p.P % 2 == pp and p.Q % 2 == qq
-    for mc in (0, 1, 2):
-        need[f"pooled, max_ctas {mc}"] = lambda c, p, mc=mc: c.pool and c.max_ctas == mc
     for fam in ("ties", "saturate"):
         need[f"{fam}, direct epilogue"] = lambda c, p, fam=fam: c.family == fam and p.splits == 1
         need[f"{fam}, split-K reduction"] = lambda c, p, fam=fam: c.family == fam and p.splits > 1

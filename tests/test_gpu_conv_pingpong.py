@@ -14,14 +14,11 @@ import pytest
 import torch
 
 from megapose6d_b200 import _abi
-from tests.test_gpu_conv_exact import (ACT, CAP, P0, P1, SMS_H100, TINY, UNIT, Conv, _conv64, _gen, _guarded, _ints,
-                                       _launch, _out_dim, _problem, _to_act, _weights)
+from tests.test_gpu_conv_exact import (ACT, CAP, DEFAULT_CONV_MODE, FORCE_PP, NEVER_PP, NO_PDL, P0, P1, SMS_H100, TINY,
+                                       UNIT, Conv, _conv64, _gen, _guarded, _ints, _launch, _out_dim, _problem, _to_act,
+                                       _weights, device_kernels, mode_fixture, set_mode)
 
 gpu = pytest.mark.gpu
-DEFAULT_CONV_MODE = 8
-NO_PDL = 512  # mode bit 9
-NEVER_PP = 134217728  # mode bit 27: never the ping-pong kernel
-FORCE_PP = 268435456  # mode bit 28: the ping-pong kernel for every convolution it can serve
 BLOCK_M = 128
 PP_STAGES = 4
 
@@ -33,7 +30,7 @@ def _items(c: Conv) -> int:
 
 def _uses_pp(c: Conv, mode: int, sms: int, out_aligned: bool = True) -> bool:
     """conv_forward's choice of convpp_wgmma_kernel for mpx_conv2d (no K split): by default C_out = 128 only."""
-    if c.cout % 128 or c.cout > 512 or c.block_n != 0 or c.splits is not None or c.pool or not out_aligned:
+    if c.cout % 128 or c.cout > 512 or c.block_n != 0 or c.splits is not None or not out_aligned:
         return False
     if mode & NEVER_PP:
         return False
@@ -83,27 +80,7 @@ CASES = [
 assert len({c.name for c in CASES}) == len(CASES)
 
 
-def _set_mode(mode):
-    _abi.lib().mpx_conv_set_mode(mode)
-
-
-@pytest.fixture
-def forced():
-    _set_mode(FORCE_PP | DEFAULT_CONV_MODE)
-    yield
-    _set_mode(DEFAULT_CONV_MODE)
-
-
-def _device_kernels(fn):
-    """Runs `fn` under torch.profiler (CUDA activities) and returns its result and the names of the kernels it launched:
-    the proof that a case ran on the kernel it is meant for, since every kernel gives the same bits."""
-    from torch.profiler import ProfilerActivity, profile
-
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        out = fn()
-        torch.cuda.synchronize()
-    names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-    return out, names
+forced = mode_fixture(FORCE_PP | DEFAULT_CONV_MODE)
 
 
 def _ran_pp(names):
@@ -120,7 +97,7 @@ def test_convpp_bit_exact(case, forced):
     if case.family == "saturate" and ACT != torch.float16:
         pytest.skip("saturation at +-65504 is the fp16 conversion")
     x, w, b, r, want = _problem(case, _gen(case.name))
-    got, names = _device_kernels(lambda: _launch(case, x, w, b, r))
+    got, names = device_kernels(lambda: _launch(case, x, w, b, r), "convpp_wgmma_kernel")
     assert _ran_pp(names) and not _ran_128row(names), names
     bad = got.float() != want.float()
     assert not bad.any(), f"{int(bad.sum())} of {bad.numel()} outputs differ, first at {bad.nonzero()[0].tolist()}"
@@ -172,10 +149,10 @@ def test_dependent_chain_on_one_stream(mode):
                                   None, _abi.ptr(a3), 0, 0, s))
 
     try:
-        _set_mode(mode | FORCE_PP)
-        _, names = _device_kernels(chain)
+        set_mode(mode | FORCE_PP)
+        _, names = device_kernels(chain, "convpp_wgmma_kernel", 3)
     finally:
-        _set_mode(DEFAULT_CONV_MODE)
+        set_mode(DEFAULT_CONV_MODE)
     assert sum("convpp_wgmma_kernel" in nm for nm in names) == 3, names
     for got, want in ((a1, y1), (a2, y2), (a3, y3)):
         assert torch.equal(got, _to_act(want))
@@ -207,10 +184,11 @@ def test_convpp_gaussian_data_within_rounding_bound(case, mode):
         y64 = torch.relu(y64)
     mag = _conv64(x.abs(), w.abs(), case.stride, case.pads) + b.abs() + (r.abs() if r is not None else 0)
     try:
-        _set_mode(mode)
-        got, names = _device_kernels(lambda: _launch(case, x.to(ACT), w, b, r.to(ACT) if r is not None else None))
+        set_mode(mode)
+        got, names = device_kernels(lambda: _launch(case, x.to(ACT), w, b, r.to(ACT) if r is not None else None),
+                                      "convpp_wgmma_kernel")
     finally:
-        _set_mode(DEFAULT_CONV_MODE)
+        set_mode(DEFAULT_CONV_MODE)
     assert _ran_pp(names), names
     err = (got.double() - y64).abs()
     bound = UNIT * y64.abs() + TINY + (k + 2) * 2.0 ** -23 * mag
@@ -253,11 +231,11 @@ def test_network_forward_bit_identical_without_pingpong():
     try:
         lib.mpx_net_set_graphs(0)
         lib.mpx_conv_set_mode(DEFAULT_CONV_MODE | NEVER_PP)
-        old, names_old = _device_kernels(lambda: eng.forward(x, h, w).clone())
+        old, names_old = device_kernels(lambda: eng.forward(x, h, w).clone())
         lib.mpx_conv_set_mode(DEFAULT_CONV_MODE)
-        new, names_new = _device_kernels(lambda: eng.forward(x, h, w).clone())
+        new, names_new = device_kernels(lambda: eng.forward(x, h, w).clone(), "convpp_wgmma_kernel", want_pp)
         lib.mpx_conv_set_mode(DEFAULT_CONV_MODE | FORCE_PP)
-        forced, names_forced = _device_kernels(lambda: eng.forward(x, h, w).clone())
+        forced, names_forced = device_kernels(lambda: eng.forward(x, h, w).clone(), "convpp_wgmma_kernel", 29)
     finally:
         lib.mpx_net_set_graphs(1)
         lib.mpx_conv_set_mode(DEFAULT_CONV_MODE)
@@ -321,7 +299,7 @@ def test_dispatch_rule_covers_the_cases():
     assert not _uses_pp(dataclasses.replace(layer2, n=576), DEFAULT_CONV_MODE | NEVER_PP, SMS_H100)
     assert not _uses_pp(dataclasses.replace(layer2, n=576), FORCE_PP | NEVER_PP, SMS_H100)
     assert _uses_pp(dataclasses.replace(layer2, n=1), FORCE_PP, SMS_H100)
-    for other in (dict(cout=64), dict(cout=192), dict(cout=640), dict(block_n=128), dict(splits=1), dict(pool=True)):
+    for other in (dict(cout=64), dict(cout=192), dict(cout=640), dict(block_n=128), dict(splits=1)):
         assert not _uses_pp(dataclasses.replace(layer2, n=576, **other), FORCE_PP, SMS_H100), other
     assert not _uses_pp(dataclasses.replace(layer2, n=576), FORCE_PP, SMS_H100, out_aligned=False)
     for other in (dict(cout=256), dict(cout=512)):  # served under bit 28 only

@@ -25,12 +25,12 @@ from megapose6d_b200.backbone import ResNet34Engine
 from oracle import resnet_ref
 from tests import helpers
 from tests import test_gpu_conv_exact as conv_exact
+from tests.test_gpu_conv_exact import DEFAULT_CONV_MODE
 
 pytestmark = pytest.mark.gpu
 ACT = _abi.act_dtype() if torch.cuda.is_available() else torch.float16
 ULP, ATOL = (2 ** -10, 2e-3) if ACT == torch.float16 else (2 ** -7, 1e-2)
 SINGLE_CTA_MODE = 11  # kernel-variant bits 0, 1 and split-K in the network (bit 3)
-DEFAULT_CONV_MODE = 8  # the library's default (include/mpx.h): split-K in the network for small batches
 RELOAD_MODE = DEFAULT_CONV_MODE | 32768  # a kernel-variant bit: no effect
 
 
@@ -522,72 +522,3 @@ def test_wide_resnet_engine_vs_oracle(backbone_str):
               f"bound={bound.min():.4g}..{bound.max():.4g}")
         assert ((got - emu).abs() <= 0.5 * bound + 2e-4).all()  # same quantisation points; 2e-4 = a fifth of an fp16 ulp at 1
         assert ((got - fp32).abs() <= bound + 1e-4).all()
-
-
-SEPARATE_POOL_MODE = DEFAULT_CONV_MODE & ~2097152  # without bit 21: stem output stored, max-pool as its own kernel
-FUSED_POOL_MODE = DEFAULT_CONV_MODE | 2097152  # bit 21: the stem's epilogue max-pools
-POOL_CASES = [
-    # name, n, h, w, r, pads, max_ctas
-    ("stem_4x4", 3, 120, 160, 4, (2, 2, 1, 1), 6),
-    ("stem_224", 2, 112, 112, 4, (2, 2, 1, 1), 0),
-    ("odd_rows_odd_cols", 3, 17, 23, 3, (1, 1, 1, 1), 2),
-    ("odd_rows", 2, 31, 40, 3, (1, 1, 1, 1), 4),
-    ("two_tiles_one_pair", 1, 12, 16, 3, (1, 1, 1, 1), 2),
-    ("stem_all_sms", 10, 120, 160, 4, (2, 2, 1, 1), 0),
-]
-
-
-@pytest.mark.parametrize("case", POOL_CASES, ids=[c[0] for c in POOL_CASES])
-def test_fused_maxpool_epilogue_equals_conv_then_maxpool(case):
-    """mpx_conv2d with relu bit 2 (the pooled epilogue: vector max-reductions into the zeroed pooled tensor) against the
-    stored convolution followed by mpx_maxpool3x3s2: the maximum is exact, so the two agree value for value (torch.equal on
-    floats: +0 == -0), for even and odd sizes, image borders and tile borders."""
-    name, n, h, w, r, pads, max_ctas = case
-    g = torch.Generator(device="cuda").manual_seed(43)
-    x = torch.randn(n, h, w, 64, device="cuda", generator=g).to(ACT)
-    wt = (torch.randn(64, r, r, 64, device="cuda", generator=g) / (r * r * 64) ** 0.5).to(ACT)
-    bias = torch.randn(64, device="cuda", generator=g)
-    ho, wo = (h - 1) // 2 + 1, (w - 1) // 2 + 1
-    lib = _abi.lib()
-    full = torch.full((n, h, w, 64), float("nan"), device="cuda", dtype=ACT)
-    _abi.check(lib.mpx_conv2d(_abi.ptr(x), n, h, w, 64, _abi.ptr(wt.view(64, -1)), _abi.ptr(bias), 64, r, r, 1, *pads, 1, None,
-                              _abi.ptr(full), 0, max_ctas, _abi.stream_ptr()))
-    want = torch.empty(n, ho, wo, 64, device="cuda", dtype=ACT)
-    _abi.check(lib.mpx_maxpool3x3s2(_abi.ptr(full), n, h, w, 64, _abi.ptr(want), _abi.stream_ptr()))
-    assert not torch.isnan(want.float()).any()
-    try:
-        for mode in (DEFAULT_CONV_MODE, RELOAD_MODE):
-            lib.mpx_conv_set_mode(mode)
-            got = torch.zeros(n, ho, wo, 64, device="cuda", dtype=ACT)
-            _abi.check(lib.mpx_conv2d(_abi.ptr(x), n, h, w, 64, _abi.ptr(wt.view(64, -1)), _abi.ptr(bias), 64, r, r, 1, *pads, 1 | 4,
-                                      None, _abi.ptr(got), 0, max_ctas, _abi.stream_ptr()))
-            torch.cuda.synchronize()
-            assert torch.equal(got.float(), want.float()), mode
-    finally:
-        lib.mpx_conv_set_mode(DEFAULT_CONV_MODE)
-    # shapes without the epilogue are refused without launching anything (the network then runs conv + max-pool)
-    assert lib.mpx_conv2d(_abi.ptr(x), n, h, w, 64, _abi.ptr(wt.view(64, -1)), _abi.ptr(bias), 64, r, r, 1, *pads, 4, None,
-                          _abi.ptr(got), 0, max_ctas, _abi.stream_ptr()) == -3  # no ReLU
-
-
-@pytest.mark.parametrize("cfg_name,n", [("coarse", 7), ("refiner", 1)])
-def test_network_with_fused_maxpool_equals_unfused(cfg_name, n):
-    """The whole forward with mode bit 21 (the stem's epilogue pools) against the stem followed by the max-pool kernel:
-    every later layer sees the same pooled tensor, so the outputs are identical."""
-    cfg = dict(coarse=helpers.COARSE_CFG, refiner=helpers.REFINER_CFG)[cfg_name]
-    sd = helpers.make_state_dict(cfg, seed=3)
-    c = helpers.n_inputs(cfg)
-    x = helpers._calibration_batch(c, 42, n=n).cuda()
-    outs = []
-    try:
-        for mode in (SEPARATE_POOL_MODE, FUSED_POOL_MODE, FUSED_POOL_MODE):
-            _abi.lib().mpx_conv_set_mode(mode)
-            eng = ResNet34Engine(sd, n_inputs=c, head=resnet_ref.head_name(sd))
-            outs.append(eng(x).clone())  # first sight of a shape runs eagerly
-            outs.append(eng(x).clone())  # ... the second captures a graph (memset node + kernels), the third replays it
-            outs.append(eng(x).clone())
-            torch.cuda.synchronize()
-    finally:
-        _abi.lib().mpx_conv_set_mode(DEFAULT_CONV_MODE)
-    for o in outs[1:]:
-        assert torch.equal(outs[0], o)
