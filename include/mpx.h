@@ -310,6 +310,9 @@ int mpx_net_destroy(mpx_net* net);
 /* mpx_net_forward and mpx_fpn_forward replay a cached CUDA graph per (buffers, shape) after the first call; 0 disables
  * that (every launch is then issued eagerly on the caller's stream). Default: enabled. */
 int mpx_net_set_graphs(int on);
+/* device workspace of mpx_net_forward for n samples of size h x w (256-byte aligned): the stem map, then 3 (5 for a
+ * pre-activation net) rotating buffers each sized for the largest activation map of layers 1-4 -- for inputs a few pixels
+ * on a side that is a deeper layer's map, not layer 1's */
 size_t mpx_net_workspace_bytes(const mpx_net* net, int n, int h, int w);
 /* d_x: network input tensor (see above) for n samples of size h x w; d_out [n, out_dim] fp32 */
 int mpx_net_forward(const mpx_net* net, const void* d_x, int n, int h, int w, float* d_out,

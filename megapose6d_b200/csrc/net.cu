@@ -280,12 +280,29 @@ void net_destroy(Net* net) {
 
 static size_t align256(size_t v) { return (v + 255) & ~static_cast<size_t>(255); }
 
+// Bytes of one rotating buffer: the largest activation map of the pooled stem output and layers 1-4, n images of the
+// pooled map hp x wp.  Each later layer halves the map (rounding up) and doubles the channels, so once a side is a few
+// pixels long a deeper map is larger than layer 1's: at 4x4 input the layer-4 map is 8 times the layer-1 map.
+static size_t rotating_buffer_bytes(int n, int hp, int wp) {
+  size_t most = 0;
+  int H = hp, W = wp;
+  for (int layer = 0; layer < 4; ++layer) {
+    if (layer > 0) {
+      H = conv_out_dim(H, 1, 1, 3, 2);
+      W = conv_out_dim(W, 1, 1, 3, 2);
+    }
+    const size_t bytes = static_cast<size_t>(n) * H * W * kLayerWidth[layer] * 2;
+    if (bytes > most) most = bytes;
+  }
+  return align256(most);
+}
+
+// [stem map][rotating buffer] x 3 (post-activation) or x 5 (pre-activation), then 1 KB of slack
 size_t net_workspace_bytes(const Net* net, int n, int h, int w) {
-  const size_t hs = h / 2, ws = w / 2;
+  const int hs = h / 2, ws = w / 2;
   const size_t stem = align256(static_cast<size_t>(n) * hs * ws * 64 * 2);
-  const size_t hp = (hs + 2 - 3) / 2 + 1, wp = (ws + 2 - 3) / 2 + 1;
-  const size_t l1 = align256(static_cast<size_t>(n) * hp * wp * 64 * 2);
-  return stem + (net != nullptr && net->preact ? 5 : 3) * l1 + 1024;
+  const int hp = (hs + 2 - 3) / 2 + 1, wp = (ws + 2 - 3) / 2 + 1;
+  return stem + (net != nullptr && net->preact ? 5 : 3) * rotating_buffer_bytes(n, hp, wp) + 1024;
 }
 
 static int net_forward_direct(const Net* net, const void* x, int n, int h, int w, float* out, void* workspace,
@@ -370,10 +387,10 @@ static int net_forward_preact(const Net* net, const void* x, int n, int h, int w
   const int hp = (hs + 2 - 3) / 2 + 1, wp = (ws + 2 - 3) / 2 + 1;
   uint8_t* base = reinterpret_cast<uint8_t*>(workspace);
   const size_t stem_bytes = align256(static_cast<size_t>(n) * hs * ws * 64 * 2);
-  const size_t l1_bytes = align256(static_cast<size_t>(n) * hp * wp * 64 * 2);
+  const size_t buf_bytes = rotating_buffer_bytes(n, hp, wp);
   void* buf_stem = base;
   void* bufs[5];
-  for (int i = 0; i < 5; ++i) bufs[i] = base + stem_bytes + i * l1_bytes;
+  for (int i = 0; i < 5; ++i) bufs[i] = base + stem_bytes + i * buf_bytes;
   const int sk = ((conv_get_mode() & MPX_CONV_NET_SPLITK) != 0 && n <= 64) ? -1 : 0;
   int rc;
   {
@@ -474,9 +491,9 @@ static int net_forward_direct(const Net* net, const void* x, int n, int h, int w
   const int hp = (hs + 2 - 3) / 2 + 1, wp = (ws + 2 - 3) / 2 + 1;
   uint8_t* base = reinterpret_cast<uint8_t*>(workspace);
   const size_t stem_bytes = align256(static_cast<size_t>(n) * hs * ws * 64 * 2);
-  const size_t l1_bytes = align256(static_cast<size_t>(n) * hp * wp * 64 * 2);
+  const size_t buf_bytes = rotating_buffer_bytes(n, hp, wp);
   void* buf_stem = base;
-  void* bufs[3] = {base + stem_bytes, base + stem_bytes + l1_bytes, base + stem_bytes + 2 * l1_bytes};
+  void* bufs[3] = {base + stem_bytes, base + stem_bytes + buf_bytes, base + stem_bytes + 2 * buf_bytes};
   // small batches (refiner iterations, final scoring): layers 2-4 split their K loop over a cluster
   const int sk = ((conv_get_mode() & MPX_CONV_NET_SPLITK) != 0 && n <= 64) ? -1 : 0;
 

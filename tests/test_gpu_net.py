@@ -160,22 +160,6 @@ def test_conv_rejects_bad_arguments():
     assert rc != 0 and b"multiple of 64" in _abi.lib().mpx_last_error()
 
 
-def test_maxpool_and_tail():
-    g = torch.Generator(device="cuda").manual_seed(0)
-    x = torch.randn(3, 30, 40, 64, device="cuda", generator=g).to(ACT)
-    out = torch.empty(3, 15, 20, 64, device="cuda", dtype=ACT)
-    _abi.check(_abi.lib().mpx_maxpool3x3s2(_abi.ptr(x), 3, 30, 40, 64, _abi.ptr(out), _abi.stream_ptr()))
-    ref = F.max_pool2d(x.float().permute(0, 3, 1, 2), 3, 2, 1).permute(0, 2, 3, 1)
-    assert torch.equal(out.float(), ref)
-    f = torch.randn(5, 80, 512, device="cuda", generator=g).to(ACT)
-    W = torch.randn(9, 512, device="cuda", generator=g) * 0.05
-    b = torch.randn(9, device="cuda", generator=g)
-    o = torch.empty(5, 9, device="cuda")
-    _abi.check(_abi.lib().mpx_avgpool_linear(_abi.ptr(f), 5, 80, 512, _abi.ptr(W), _abi.ptr(b), 9, _abi.ptr(o), _abi.stream_ptr()))
-    ref = f.float().mean(dim=1) @ W.t() + b
-    assert torch.allclose(o, ref, rtol=1e-4, atol=1e-4)
-
-
 @pytest.mark.parametrize("cfg_name", ["coarse", "refiner", "refiner_rgbd"])
 def test_resnet34_engine_vs_oracle(cfg_name):
     cfg = dict(coarse=helpers.COARSE_CFG, refiner=helpers.REFINER_CFG, refiner_rgbd=helpers.REFINER_RGBD_CFG)[cfg_name]

@@ -197,3 +197,107 @@ def make_state_dict(cfg, seed=0):
         sd[head + ".bias"] = -offset
     _SD_CACHE[key] = dict(sd)
     return sd
+
+
+def integer_state_dict(n_inputs: int, head: str = "views_logits_head", head_dim: int = 512, readout: bool = True,
+                       seed: int = 0, backbone_str: str = "vanilla_resnet34", nnz: int = 2,
+                       stem_nnz: int = 4) -> Dict[str, torch.Tensor]:
+    """A state dict in the checkpoint layout (either backbone family) on which every value of the engine's plan is an
+    integer, so that its fp32 accumulation is exact in any order and it must equal the float64 plan of
+    oracle/net_plan_ref.py bit for bit on inputs of small integers:
+      * every convolution: `nnz` non-zero weights per output channel (`stem_nnz` for the stem, on real taps of real input
+        channels), the rest zero;
+      * every BatchNorm folded into a convolution (stored in float64): gamma = 2^e sqrt(var + eps) with e in {-1, 0, 1} per
+        channel, so that the folded scale is exactly 2^e, an integer beta and an even integer mean.  The raw weights are
+        +-1, and +-2 where e = -1: the folded weights are integers (+-1, +-2), and so is the folded bias;
+      * the pre-activation affine (WideResNet bn1): scale in {0.5, 1, 2} and an integer shift, both varying by channel.  The
+        channels scaled by 0.5 are a fixed set per layer on which every producer of the residual stream writes even values
+        (folded stem weights +-2 and an even bias, conv2 and downsample weights +-2), so that the affine stays integral;
+      * `readout` (head_dim 512): fc = I with zero bias (post-activation), and the head a signed permutation scaled by 2^e
+        per row with zero bias -- every pooled channel reaches one output unchanged up to a power of two.  Otherwise the
+        head (and the fc) get Gaussian weights, as init_state_dict.
+    net_plan_ref.forward asserts for every convolution and the pooled sums that the partial sums stay below 2^24."""
+    g = torch.Generator().manual_seed(seed)
+    sd: Dict[str, torch.Tensor] = {}
+    wide = backbone_str in WIDE_LAYERS
+
+    def ints(lo, hi, shape):
+        return torch.randint(lo, hi + 1, shape, generator=g).double()
+
+    def conv(name, co, ci, k, nz, mag=None):
+        """+-mag[o] at nz random taps of output channel o (mag: per channel, default 1)."""
+        w = torch.zeros(co, ci * k * k, dtype=torch.float64)
+        idx = torch.stack([torch.randperm(ci * k * k, generator=g)[:nz] for _ in range(co)])
+        sign = ints(0, 1, (co, nz)) * 2 - 1
+        w.scatter_(1, idx, sign * (mag.view(-1, 1) if mag is not None else 1.0))
+        sd[name + ".weight"] = w.view(co, ci, k, k)
+
+    def folded_conv(name, bn_name, co, ci, k, nz, even=None):
+        """Convolution + BatchNorm with integer folded weights and bias; `even` channels get even outputs (e = 1)."""
+        e = ints(-1, 1, (co,))
+        beta = ints(-2, 2, (co,))
+        if even is not None:
+            e[even] = 1.0
+            beta[even] = 2 * torch.round(beta[even] / 2)
+        conv(name, co, ci, k, nz, mag=torch.where(e < 0, 2.0, 1.0))
+        var = 0.5 + torch.rand(co, generator=g, dtype=torch.float64)
+        sd[bn_name + ".weight"] = 2.0 ** e * torch.sqrt(var + BN_EPS)
+        sd[bn_name + ".bias"] = beta
+        sd[bn_name + ".running_mean"] = 2 * ints(-1, 1, (co,))
+        sd[bn_name + ".running_var"] = var
+        sd[bn_name + ".num_batches_tracked"] = torch.tensor(1)
+
+    def affine(name, c, halved):
+        """bn1 of a pre-activation block: scale 0.5 on `halved`, else 1 or 2; integer shift."""
+        scale = torch.where(ints(0, 1, (c,)) > 0, 2.0, 1.0).double()
+        scale[halved] = 0.5
+        var = 0.5 + torch.rand(c, generator=g, dtype=torch.float64)
+        sd[name + ".weight"] = scale * torch.sqrt(var + BN_EPS)
+        sd[name + ".bias"] = ints(-3, 3, (c,))
+        sd[name + ".running_mean"] = torch.zeros(c, dtype=torch.float64)
+        sd[name + ".running_var"] = var
+        sd[name + ".num_batches_tracked"] = torch.tensor(1)
+
+    inplanes = 64
+    if wide:
+        halved = {w: torch.randperm(w, generator=g)[:w // 3] for w in WIDTHS}  # per stream width
+        folded_conv("backbone.conv1", "backbone.bn1", 64, n_inputs, 5, stem_nnz, even=halved[64])
+        for li, (nb, width) in enumerate(zip(WIDE_LAYERS[backbone_str], WIDTHS)):
+            two = torch.ones(width, dtype=torch.float64)
+            two[halved[width]] = 2.0
+            for b in range(nb):
+                p = f"backbone.layer{li + 1}.{b}"
+                stride = 2 if (b == 0 and li > 0) else 1
+                affine(p + ".bn1", inplanes, halved[inplanes])
+                folded_conv(p + ".conv1", p + ".bn2", width, inplanes, 3, nnz)
+                conv(p + ".conv2", width, width, 3, nnz, mag=two)
+                if stride != 1 or inplanes != width:
+                    conv(p + ".downsample", width, inplanes, 1, 1, mag=two)
+                inplanes = width
+    else:
+        folded_conv("backbone.conv1", "backbone.bn1", 64, n_inputs, 7, stem_nnz)
+        for li, (nb, width) in enumerate(zip(LAYERS, WIDTHS)):
+            for b in range(nb):
+                p = f"backbone.layer{li + 1}.{b}"
+                stride = 2 if (b == 0 and li > 0) else 1
+                folded_conv(p + ".conv1", p + ".bn1", width, inplanes, 3, nnz)
+                folded_conv(p + ".conv2", p + ".bn2", width, width, 3, nnz)
+                if stride != 1 or inplanes != width:
+                    folded_conv(p + ".downsample.0", p + ".downsample.1", width, inplanes, 1, 1)
+                inplanes = width
+    if readout:
+        assert head_dim == 512
+        if not wide:
+            sd["backbone.fc.weight"] = torch.eye(512, dtype=torch.float64)
+            sd["backbone.fc.bias"] = torch.zeros(512, dtype=torch.float64)
+        perm = torch.randperm(512, generator=g)
+        scale = (2.0 ** ints(-1, 1, (512,))) * (ints(0, 1, (512,)) * 2 - 1)
+        sd[head + ".weight"] = torch.zeros(512, 512, dtype=torch.float64).index_put_((torch.arange(512), perm), scale)
+        sd[head + ".bias"] = torch.zeros(512, dtype=torch.float64)
+    else:
+        if not wide:
+            sd["backbone.fc.weight"] = torch.randn(512, 512, generator=g, dtype=torch.float64) * (1.0 / 512) ** 0.5
+            sd["backbone.fc.bias"] = 0.1 * torch.randn(512, generator=g, dtype=torch.float64)
+        sd[head + ".weight"] = torch.randn(head_dim, 512, generator=g, dtype=torch.float64) * (1.0 / 512) ** 0.5
+        sd[head + ".bias"] = 0.1 * torch.randn(head_dim, generator=g, dtype=torch.float64)
+    return sd
