@@ -376,7 +376,8 @@ int mpx_mask_paste(const float* d_logits, const int64_t* d_labels, const float* 
                    float* const* h_masks, void* stream);
 
 /* ---- BOP 2019 pose errors ------------------------------------------------------------------------
- * The pose-error functions of the BOP toolkit (bop_toolkit_lib/pose_error.py: vsd, mssd, mspd, add, adi), vendored by the
+ * The pose-error functions of the BOP toolkit (bop_toolkit_lib/pose_error.py: vsd, mssd, mspd, add, adi, cus, proj, re,
+ * te), vendored by the
  * reference under deps/bop_toolkit_challenge; megapose6d_b200/bop_eval.py drives them.  Lengths are millimetres.
  *
  * mpx_bop_vsd: Visible Surface Discrepancy with the "step" cost and "bop19" visibility.  Pair p compares estimate render
@@ -434,6 +435,29 @@ int mpx_bop_point_errors(int kind, int n_pairs, int n_models, const double* d_pt
 int mpx_bop_gt_info(int n_gt, int h, int w, const uint16_t* d_depth_test, int n_img, const float* d_depth_scale,
                     const double* d_K, const float* d_depth_gt_large, const int32_t* d_img_idx, float delta,
                     int64_t* d_counts, int32_t* d_bbox, uint8_t* d_mask, uint8_t* d_mask_visib, void* stream);
+
+/* mpx_bop_cus: Complement over Union of the two silhouettes (pose_error.cus: depth > 0) of estimate render
+ * d_depth_est[d_est_idx[p]] and ground-truth render d_depth_gt[d_gt_idx[p]], in mpx_bop_vsd's layout ([n_est|n_gt, h, w]
+ * float32 METRES, 0 = no surface; renders shared by every pair that names them).  Outputs: d_counts [n_pairs, 2] int64 =
+ * {intersection, union}, d_err [n_pairs] float64 = 1 - intersection / union in the toolkit's float64 expression (bit-
+ * identical to it on the same renders), 1.0 when the union is empty, NaN for a pair whose indices are out of range.  The
+ * counts are warp / CTA sums with one 64-bit atomic per counter per CTA: they do not depend on the launch shape.  Refused
+ * before any launch: n_pairs < 0, n_est or n_gt < 1, empty images, h * w >= 2^31, a NULL or non-device pointer. */
+int mpx_bop_cus(int n_pairs, int h, int w, const float* d_depth_est, int n_est, const float* d_depth_gt, int n_gt,
+                const int32_t* d_est_idx, const int32_t* d_gt_idx, int64_t* d_counts, double* d_err, void* stream);
+
+/* mpx_bop_pose_errors: per pair of poses d_pose_est / d_pose_gt [n_pairs, 12] float64 (R row-major, t in mm), any of
+ *   d_proj [n_pairs]  pose_error.proj: mean over the points of model d_model_idx[p] (mpx_bop_point_errors' point store)
+ *                     of the distance between their projections under d_K [n_pairs, 9] (px), P = K [R|t] formed first as
+ *                     misc.project_pts does, summed in the fixed-order block reduction of MPX_BOP_ADD
+ *   d_re [n_pairs]    pose_error.re: acos(0.5 (trace(R_est inv(R_gt)) - 1)) in degrees, the cosine clipped to [-1, 1]
+ *   d_te [n_pairs]    pose_error.te: |t_gt - t_est| (mm)
+ * float64; a NULL output is skipped, and the point store, model indices and K are only read (and required) with d_proj.  A
+ * pair with an unknown model or no points gets a NaN PROJ.  Refused before any launch: n_pairs < 0, n_models < 1 (with
+ * d_proj), a NULL required or a non-device pointer. */
+int mpx_bop_pose_errors(int n_pairs, int n_models, const double* d_pts, const int64_t* d_pt_offsets, long long n_pts_total,
+                        const int32_t* d_model_idx, const double* d_pose_est, const double* d_pose_gt, const double* d_K,
+                        double* d_proj, double* d_re, double* d_te, void* stream);
 
 /* ---- depth refinement (TEASER++) ----------------------------------------------------------------------------------
  * Replaces the per-prediction host path of TeaserppRefiner.refine_poses / compute_teaserpp_refinement

@@ -80,6 +80,8 @@ def _declare(lib: ctypes.CDLL) -> None:
     lib.mpx_bop_point_errors.argtypes = [c_int, c_int, c_int, vp, vp, ctypes.c_longlong, vp, vp, ctypes.c_longlong, vp, vp,
                                          vp, vp, vp, vp, vp]
     lib.mpx_bop_gt_info.argtypes = [c_int, c_int, c_int, vp, c_int, vp, vp, vp, vp, c_float, vp, vp, vp, vp, vp]
+    lib.mpx_bop_cus.argtypes = [c_int, c_int, c_int, vp, c_int, vp, c_int, vp, vp, vp, vp, vp]
+    lib.mpx_bop_pose_errors.argtypes = [c_int, c_int, vp, vp, ctypes.c_longlong, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.mpx_teaser_points.argtypes = [c_int, c_int, c_int, vp, vp, c_int, vp, vp, c_int, c_float, vp, vp, vp, vp, vp, vp]
     lib.mpx_teaser_fps_workspace_bytes.argtypes = [c_int, c_int]
     lib.mpx_teaser_fps_workspace_bytes.restype = c_size_t
@@ -113,7 +115,7 @@ EXPORTS = [
     "mpx_net_input_bytes", "mpx_conv2d", "mpx_conv2d_splitk", "mpx_conv_set_mode", "mpx_maxpool3x3s2", "mpx_avgpool_linear",
     "mpx_net_create", "mpx_net_create_preact", "mpx_net_destroy", "mpx_net_set_graphs", "mpx_net_workspace_bytes", "mpx_net_forward",
     "mpx_fpn_create", "mpx_fpn_destroy", "mpx_fpn_workspace_bytes", "mpx_fpn_forward", "mpx_mask_paste",
-    "mpx_bop_vsd", "mpx_bop_point_errors", "mpx_bop_gt_info",
+    "mpx_bop_vsd", "mpx_bop_point_errors", "mpx_bop_gt_info", "mpx_bop_cus", "mpx_bop_pose_errors",
     "mpx_teaser_points", "mpx_teaser_fps_workspace_bytes", "mpx_teaser_fps", "mpx_teaser_graph",
     "mpx_teaser_clique_workspace_bytes", "mpx_teaser_max_clique", "mpx_teaser_solve",
 ]

@@ -10,7 +10,13 @@ Depth renders come from the engine's rasteriser (`BatchRenderer.render(render_de
 the per-pixel VSD reduction and the per-point MSSD / MSPD / ADD / ADI reductions are the kernels of csrc/bop_eval.cu
 (include/mpx.h: mpx_bop_vsd, mpx_bop_point_errors).
 
+The toolkit's other error types (scripts/eval_calc_errors.py: ad, add, adi, cus, proj, re, te, rete) are scored as its
+scripts/eval_calc_scores.py does with n_top = -1 and visib_gt_min = -1: a recall per type at its own threshold
+(LOCALIZATION_THRESHOLDS, overridable per type), with per-object and per-scene recalls.  CUS uses the VSD renders
+(mpx_bop_cus), PROJ / RE / TE the point store (mpx_bop_pose_errors).
+
     python -m megapose6d_b200.bop_eval <dataset_dir> <results.csv> [--split test] [--errors-out DIR]
+        [--error-types ad,add,adi,cus,proj,re,te,rete] [--correct-th te=50 ...] [--symmetric-obj-ids 10,11]
 """
 from __future__ import annotations
 
@@ -33,6 +39,15 @@ VSD_DELTAS = {"itodd": 5}
 VSD_DELTA_DEFAULT = 15
 MAX_SYM_DISC_STEP = 0.01
 KINDS = {"mssd": 0, "mspd": 1, "add": 2, "adi": 3}
+BOP19_TYPES = ("vsd", "mssd", "mspd")
+# The toolkit's other error types (scripts/eval_calc_errors.py) and their default correctness thresholds
+# (scripts/eval_calc_scores.py): one threshold per error element.  ad / add / adi are fractions of the diameter, cus a
+# fraction of the union, proj pixels, re degrees.  te is compared in the unit of its errors, mm, although the toolkit
+# labels its thresholds "cm": te 5 and the second element of rete 5 mean 5 mm.
+LOCALIZATION_THRESHOLDS = {"ad": [0.1], "add": [0.1], "adi": [0.1], "cus": [0.5], "proj": [5.0], "re": [5.0], "te": [5.0],
+                           "rete": [5.0, 5.0]}
+ERROR_TYPES = BOP19_TYPES + ("add", "adi") + tuple(t for t in LOCALIZATION_THRESHOLDS if t not in ("add", "adi"))
+NORMALIZED_BY_DIAMETER = ("ad", "add", "adi")
 
 
 # ------------------------------------------------------------------------------------------------------------ split reader
@@ -119,6 +134,22 @@ class BopSplit:
         return np.asarray(self.scene_camera[scene_id][im_id]["cam_K"], np.float64).reshape(3, 3)
 
 
+def split_scene_ids(split: BopSplit) -> List[int]:
+    """Every scene of the split: its numbered scene directories and the scenes of its targets (the toolkit's
+    `dataset_params` lists a dataset's scenes by hand)."""
+    ids = {t["scene_id"] for t in split.targets}
+    if split.root is not None and (Path(split.root) / split.split).is_dir():
+        ids |= {int(d.name) for d in (Path(split.root) / split.split).iterdir() if d.is_dir() and d.name.isdigit()}
+    return sorted(ids)
+
+
+def default_symmetric_obj_ids(models_info: Dict[int, dict]) -> List[int]:
+    """The objects whose models_info entry lists discrete or continuous symmetries.  The toolkit keeps a hand-written
+    per-dataset table instead (`dataset_params`); the two can differ."""
+    return sorted(o for o, info in models_info.items()
+                  if info.get("symmetries_discrete") or info.get("symmetries_continuous"))
+
+
 def load_split(dataset_dir: Union[str, Path], split: str = "test", targets_filename: str = "test_targets_bop19.json") -> BopSplit:
     from .meshes import load_ply
 
@@ -190,6 +221,20 @@ def vsd_from_depths(depth_test: torch.Tensor, depth_scale: torch.Tensor, K: torc
     return err, counts
 
 
+def cus_from_depths(depth_est: torch.Tensor, depth_gt: torch.Tensor, est_idx: torch.Tensor, gt_idx: torch.Tensor):
+    """mpx_bop_cus on device tensors: depth_est [E,h,w] / depth_gt [G,h,w] float32 metres, index tensors [P] int32.
+    Returns (errors [P] float64, counts [P, 2] int64 = (intersection, union)), on the device, without a host sync."""
+    n = int(est_idx.numel())
+    dev = depth_est.device
+    h, w = depth_est.shape[-2:]
+    err = torch.empty(n, dtype=torch.float64, device=dev)
+    counts = torch.empty(n, 2, dtype=torch.int64, device=dev)
+    _abi.check(_abi.lib().mpx_bop_cus(n, h, w, _abi.ptr(depth_est), depth_est.shape[0], _abi.ptr(depth_gt),
+                                      depth_gt.shape[0], _abi.ptr(est_idx), _abi.ptr(gt_idx), _abi.ptr(counts),
+                                      _abi.ptr(err), _abi.stream_ptr()))
+    return err, counts
+
+
 class PointStore:
     """Model points (float64 mm) and symmetry transforms of several models, concatenated on the device."""
 
@@ -213,6 +258,19 @@ class PointStore:
             _abi.ptr(self.sym_off), self.syms.shape[0], _abi.ptr(model_idx), _abi.ptr(pose_est), _abi.ptr(pose_gt),
             _abi.ptr(K), _abi.ptr(err), _abi.ptr(arg), _abi.stream_ptr()))
         return err, arg
+
+    def pose_errors(self, pose_est: torch.Tensor, pose_gt: torch.Tensor, model_idx: Optional[torch.Tensor] = None,
+                    K: Optional[torch.Tensor] = None, types: Iterable[str] = ("proj", "re", "te")) -> Dict[str, torch.Tensor]:
+        """mpx_bop_pose_errors: pose_* [P, 12] float64 (R row-major, t mm); model_idx [P] int32 and K [P, 3, 3] float64
+        for proj.  Returns {type: [P] float64} on the device for the requested types (proj px, re degrees, te mm)."""
+        types = tuple(types)
+        n = int(pose_est.shape[0])
+        out = {t: torch.empty(n, dtype=torch.float64, device=self.pts.device) for t in ("proj", "re", "te") if t in types}
+        _abi.check(_abi.lib().mpx_bop_pose_errors(
+            n, self.n_models, _abi.ptr(self.pts), _abi.ptr(self.pt_off), self.pts.shape[0], _abi.ptr(model_idx),
+            _abi.ptr(pose_est), _abi.ptr(pose_gt), _abi.ptr(K), _abi.ptr(out.get("proj")), _abi.ptr(out.get("re")),
+            _abi.ptr(out.get("te")), _abi.stream_ptr()))
+        return out
 
 
 def _pose12(R: np.ndarray, t: np.ndarray) -> np.ndarray:
@@ -281,8 +339,92 @@ def recall(split: BopSplit, rows: Sequence[dict], errors: np.ndarray, threshold:
     return tps / float(tars)
 
 
-def score_errors(split: BopSplit, errors_df, ests: Sequence[dict], types=("vsd", "mssd", "mspd")) -> dict:
-    """Average recalls of an error table (BopEvaluator.errors) under the bop19 thresholds."""
+def match_errors(rows: Sequence[dict], errors: np.ndarray, thresholds: Sequence[float],
+                 valid: Dict[Tuple[int, int], List[bool]]) -> set:
+    """The toolkit's `pose_matching.match_poses` for errors of one or more elements (rete: [re, te]), over every (image,
+    object): by decreasing score (stable), each estimate takes the valid, unmatched gt whose error is strictly below the
+    best so far in EVERY element, starting from the thresholds.  errors [n_rows, n_elems] (or [n_rows]) already
+    normalised.  Returns the matched (scene_id, im_id, gt_id)."""
+    ths = [float(x) for x in thresholds]
+    errors = np.asarray(errors, np.float64).reshape(len(rows), -1 if len(rows) else len(ths))
+    if errors.shape[1] != len(ths):
+        raise ValueError(f"{errors.shape[1]} error elements but {len(ths)} thresholds")
+    by_est: Dict[Tuple[int, int, int, int], List[Tuple[int, np.ndarray]]] = {}
+    for r, e in zip(rows, errors):
+        by_est.setdefault((r["scene_id"], r["im_id"], r["obj_id"], r["est_id"]), []).append((r["gt_id"], e))
+    score = {(r["scene_id"], r["im_id"], r["obj_id"], r["est_id"]): r["score"] for r in rows}
+    groups: Dict[Tuple[int, int, int], List[Tuple[float, List[Tuple[int, np.ndarray]]]]] = {}
+    for key, errs in by_est.items():
+        groups.setdefault(key[:3], []).append((score[key], errs))
+    matched = set()
+    for (scene_id, im_id, _), ests in groups.items():
+        mask = valid.get((scene_id, im_id))
+        if mask is None:
+            continue
+        for _, errs in sorted(ests, key=lambda e: e[0], reverse=True):
+            best_gt, best = -1, ths
+            for gt_id, e in errs:
+                if mask[gt_id] and (scene_id, im_id, gt_id) not in matched and all(e[j] < best[j] for j in range(len(ths))):
+                    best_gt, best = gt_id, e
+            if best_gt >= 0:
+                matched.add((scene_id, im_id, best_gt))
+    return matched
+
+
+def localization_scores(split: BopSplit, matched: set, valid: Dict[Tuple[int, int], List[bool]]) -> dict:
+    """The toolkit's `score.calc_localization_scores` with n_top = -1: recall over the valid gts of the target images,
+    per object (every model of models_info) and per scene (every scene of the split); an object or scene without targets
+    has recall 0 and counts in the means."""
+    obj_ids, scene_ids = sorted(split.models_info), split_scene_ids(split)
+    obj_tars, obj_tps = {o: 0 for o in obj_ids}, {o: 0 for o in obj_ids}
+    scene_tars, scene_tps = {s: 0 for s in scene_ids}, {s: 0 for s in scene_ids}
+    gt_count = tars = tps = 0
+    for (scene_id, im_id), mask in valid.items():
+        gts = split.scene_gt[scene_id][im_id]
+        gt_count += len(gts)
+        for gt_id, ok in enumerate(mask):
+            if not ok:
+                continue
+            o = gts[gt_id]["obj_id"]
+            tars += 1
+            obj_tars[o] += 1
+            scene_tars[scene_id] += 1
+            if (scene_id, im_id, gt_id) in matched:
+                tps += 1
+                obj_tps[o] += 1
+                scene_tps[scene_id] += 1
+
+    def calc_recall(tp: int, n: int) -> float:
+        return tp / float(n) if n else 0.0
+
+    obj_recalls = {o: calc_recall(obj_tps[o], obj_tars[o]) for o in obj_ids}
+    scene_recalls = {s: calc_recall(scene_tps[s], scene_tars[s]) for s in scene_ids}
+    return dict(recall=calc_recall(tps, tars), obj_recalls=obj_recalls,
+                mean_obj_recall=float(np.mean(list(obj_recalls.values()))), scene_recalls=scene_recalls,
+                mean_scene_recall=float(np.mean(list(scene_recalls.values()))), gt_count=gt_count, targets_count=tars,
+                tp_count=tps)
+
+
+def resolve_thresholds(thresholds: Optional[Dict[str, Sequence[float]]] = None) -> Dict[str, List[float]]:
+    """LOCALIZATION_THRESHOLDS with per-type overrides (the toolkit's --correct_th_<type>), one value per error element."""
+    out = {t: list(v) for t, v in LOCALIZATION_THRESHOLDS.items()}
+    for t, v in (thresholds or {}).items():
+        if t not in out:
+            raise ValueError(f"no correctness threshold for error type {t!r} (one of {', '.join(out)})")
+        v = [float(x) for x in (v if isinstance(v, (list, tuple, np.ndarray)) else [v])]
+        if len(v) != len(out[t]):
+            raise ValueError(f"{t} takes {len(out[t])} threshold(s), got {v}")
+        out[t] = v
+    return out
+
+
+def score_errors(split: BopSplit, errors_df, ests: Sequence[dict], types=("vsd", "mssd", "mspd"),
+                 thresholds: Optional[Dict[str, Sequence[float]]] = None) -> dict:
+    """Average recalls of an error table (BopEvaluator.errors) under the bop19 thresholds, then, for each of the other
+    types asked for (LOCALIZATION_THRESHOLDS), the toolkit's score dict under `<type>`: recall, obj_recalls,
+    mean_obj_recall, scene_recalls, mean_scene_recall, gt_count, targets_count, tp_count.  ad / add / adi errors are
+    divided by the diameter; rete is matched on the re and te columns together.  thresholds overrides the defaults per
+    type; te thresholds are in mm (the unit of the te errors), as the toolkit compares them."""
     valid = gt_valid_masks(split)
     rows = errors_df[["scene_id", "im_id", "obj_id", "est_id", "gt_id", "score"]].to_dict("records")
     out: dict = {}
@@ -309,6 +451,17 @@ def score_errors(split: BopSplit, errors_df, ests: Sequence[dict], types=("vsd",
     if all(k in ar for k in ("vsd", "mssd", "mspd")):
         out["bop19_average_recall"] = float(np.mean([ar["vsd"], ar["mssd"], ar["mspd"]]))
     out["bop19_average_time_per_image"] = average_time_per_image(ests)
+    ths = resolve_thresholds(thresholds)
+    for t in types:
+        if t not in ths:
+            continue
+        if t == "rete":
+            e = errors_df[["re", "te"]].to_numpy(np.float64)
+        else:
+            e = errors_df[t].to_numpy(np.float64)
+            if t in NORMALIZED_BY_DIAMETER:
+                e = e / np.array([float(split.models_info[o]["diameter"]) for o in errors_df["obj_id"]], np.float64)
+        out[t] = localization_scores(split, match_errors(rows, e, ths[t], valid), valid)
     return out
 
 
@@ -331,15 +484,22 @@ class BopEvaluator:
     """BOP 2019 evaluation of pose estimates on one split of a BOP dataset, on the device.
 
     `errors(results)` -> one row per (selected estimate, ground truth of the same object in its image);
-    `evaluate(results)` -> the bop19 average recalls, the recalls per threshold and the mean time per image."""
+    `evaluate(results)` -> the bop19 average recalls, the recalls per threshold and the mean time per image, and the
+    toolkit's score dict of each other error type asked for (ERROR_TYPES).
+
+    `ad` takes ADI for the objects of `symmetric_obj_ids` and ADD for the others; by default these are the objects whose
+    models_info entry lists symmetries (default_symmetric_obj_ids), which may differ from the toolkit's per-dataset table."""
 
     def __init__(self, dataset_dir: Union[str, Path], split: str = "test", device: str = "cuda",
-                 vsd_delta: Optional[float] = None, max_renders_per_chunk: int = 256):
+                 vsd_delta: Optional[float] = None, max_renders_per_chunk: int = 256,
+                 symmetric_obj_ids: Optional[Iterable[int]] = None):
         self.split = load_split(dataset_dir, split)
         self.device = torch.device(device)
         name = Path(dataset_dir).resolve().name
         self.vsd_delta = vsd_delta if vsd_delta is not None else VSD_DELTAS.get(name, VSD_DELTA_DEFAULT)
         self.max_renders = max_renders_per_chunk
+        self.symmetric_obj_ids = (sorted(int(o) for o in symmetric_obj_ids) if symmetric_obj_ids is not None
+                                  else default_symmetric_obj_ids(self.split.models_info))
         self.obj_ids = sorted(self.split.models)
         self.model_index = {o: i for i, o in enumerate(self.obj_ids)}
         self._renderer = None
@@ -390,8 +550,14 @@ class BopEvaluator:
                                      _t_gt=np.asarray(gt["cam_t_m2c"], np.float64).reshape(3)))
         return rows
 
-    def _vsd(self, sel: Sequence[dict], rows: List[dict]) -> np.ndarray:
-        out = np.ones((len(rows), len(VSD_TAUS)), np.float64)
+    def _vsd(self, sel: Sequence[dict], rows: List[dict], types: Sequence[str] = ("vsd",)) -> Dict[str, np.ndarray]:
+        """The errors that need renders, vsd and / or cus, from one set of render chunks: {type: errors}.  Both are 1.0
+        without rendering where the projections of the bounding spheres do not overlap."""
+        out = {}
+        if "vsd" in types:
+            out["vsd"] = np.ones((len(rows), len(VSD_TAUS)), np.float64)
+        if "cus" in types:
+            out["cus"] = np.ones(len(rows), np.float64)
         todo = [k for k, r in enumerate(rows)
                 if spheres_projections_overlap(0.5 * self.split.models_info[r["obj_id"]]["diameter"], sel[r["_est"]]["t"],
                                                r["_t_gt"])]
@@ -410,7 +576,7 @@ class BopEvaluator:
             self._vsd_chunk(sel, rows, chunk, out)
         return out
 
-    def _vsd_chunk(self, sel, rows, chunk: List[int], out: np.ndarray) -> None:
+    def _vsd_chunk(self, sel, rows, chunk: List[int], out: Dict[str, np.ndarray]) -> None:
         by_size: Dict[Tuple[int, int], List[int]] = {}
         depths: Dict[Tuple[int, int], np.ndarray] = {}
         for k in chunk:
@@ -432,27 +598,34 @@ class BopEvaluator:
             d_gt = self.render_depth([gt_rows[g]["obj_id"] for g in gt_keys], [gt_rows[g]["_R_gt"] for g in gt_keys],
                                      [gt_rows[g]["_t_gt"] for g in gt_keys], [self.split.K(g[0], g[1]) for g in gt_keys],
                                      (h, w))
-            test = torch.from_numpy(np.stack([depths[key] for key in imgs]).view(np.int16)).to(self.device)
-            scale = torch.tensor([self.split.scene_camera[s][i]["depth_scale"] for s, i in imgs], dtype=torch.float32,
-                                 device=self.device)
-            K = torch.from_numpy(np.stack([self.split.K(s, i) for s, i in imgs])).to(self.device)
             idx = lambda keys: torch.tensor(keys, dtype=torch.int32, device=self.device)  # noqa: E731
-            diam = torch.tensor([float(self.split.models_info[rows[k]["obj_id"]]["diameter"]) for k in ks],
-                                dtype=torch.float64, device=self.device)
-            err, _ = vsd_from_depths(test, scale, K, d_est, d_gt, idx([est_i[rows[k]["_est"]] for k in ks]),
-                                     idx([gt_i[(rows[k]["scene_id"], rows[k]["im_id"], rows[k]["gt_id"])] for k in ks]),
-                                     idx([im_i[(rows[k]["scene_id"], rows[k]["im_id"])] for k in ks]), diam,
-                                     self.vsd_delta)
-            out[ks] = err.cpu().numpy()
+            e_idx = idx([est_i[rows[k]["_est"]] for k in ks])
+            g_idx = idx([gt_i[(rows[k]["scene_id"], rows[k]["im_id"], rows[k]["gt_id"])] for k in ks])
+            if "vsd" in out:
+                test = torch.from_numpy(np.stack([depths[key] for key in imgs]).view(np.int16)).to(self.device)
+                scale = torch.tensor([self.split.scene_camera[s][i]["depth_scale"] for s, i in imgs],
+                                     dtype=torch.float32, device=self.device)
+                K = torch.from_numpy(np.stack([self.split.K(s, i) for s, i in imgs])).to(self.device)
+                diam = torch.tensor([float(self.split.models_info[rows[k]["obj_id"]]["diameter"]) for k in ks],
+                                    dtype=torch.float64, device=self.device)
+                err, _ = vsd_from_depths(test, scale, K, d_est, d_gt, e_idx, g_idx,
+                                         idx([im_i[(rows[k]["scene_id"], rows[k]["im_id"])] for k in ks]), diam,
+                                         self.vsd_delta)
+                out["vsd"][ks] = err.cpu().numpy()
+            if "cus" in out:
+                err, _ = cus_from_depths(d_est, d_gt, e_idx, g_idx)
+                out["cus"][ks] = err.cpu().numpy()
 
-    def _point(self, kind: str, sel, rows: List[dict]) -> Tuple[np.ndarray, np.ndarray]:
+    def _point(self, kind: str, sel, rows: List[dict], todo: Optional[List[int]] = None) -> Tuple[np.ndarray, np.ndarray]:
+        """Errors of `kind` for rows `todo` (default: every row that the toolkit computes), inf elsewhere."""
         err = np.full(len(rows), np.inf)
         arg = np.full(len(rows), -1, np.int64)
         if kind == "mspd":
             todo = list(range(len(rows)))
         else:  # the toolkit gives inf without computing when the centres are a diameter or more apart
-            todo = [k for k, r in enumerate(rows)
-                    if np.linalg.norm(sel[r["_est"]]["t"] - r["_t_gt"]) < self.split.models_info[r["obj_id"]]["diameter"]]
+            todo = [k for k in (range(len(rows)) if todo is None else todo)
+                    if np.linalg.norm(sel[rows[k]["_est"]]["t"] - rows[k]["_t_gt"])
+                    < self.split.models_info[rows[k]["obj_id"]]["diameter"]]
         if not todo:
             return err, arg
         dev = self.device
@@ -467,46 +640,142 @@ class BopEvaluator:
         arg[todo] = a.cpu().numpy()
         return err, arg
 
-    def errors(self, results, types: Iterable[str] = ("vsd", "mssd", "mspd")):
+    def _ad(self, sel, rows: List[dict]) -> np.ndarray:
+        """ADI for the rows of symmetric objects, ADD for the others (gated as ADD / ADI)."""
+        sym = set(self.symmetric_obj_ids)
+        e_adi, _ = self._point("adi", sel, rows, [k for k, r in enumerate(rows) if r["obj_id"] in sym])
+        e_add, _ = self._point("add", sel, rows, [k for k, r in enumerate(rows) if r["obj_id"] not in sym])
+        return np.where([r["obj_id"] in sym for r in rows], e_adi, e_add)
+
+    def _pose(self, types: Sequence[str], sel, rows: List[dict]) -> Dict[str, np.ndarray]:
+        """proj (px), re (degrees) and te (mm) of every row, never gated."""
+        if not rows:
+            return {t: np.zeros(0) for t in types}
+        dev = self.device
+        pe = torch.from_numpy(np.stack([_pose12(sel[r["_est"]]["R"], sel[r["_est"]]["t"]) for r in rows])).to(dev)
+        pg = torch.from_numpy(np.stack([_pose12(r["_R_gt"], r["_t_gt"]) for r in rows])).to(dev)
+        m = K = None
+        if "proj" in types:
+            m = torch.tensor([self.model_index[r["obj_id"]] for r in rows], dtype=torch.int32, device=dev)
+            K = torch.from_numpy(np.stack([self.split.K(r["scene_id"], r["im_id"]) for r in rows])).to(dev)
+        return {t: v.cpu().numpy() for t, v in self.points.pose_errors(pe, pg, m, K, types).items()}
+
+    def errors(self, results, types: Iterable[str] = BOP19_TYPES):
         """pandas DataFrame, one row per (selected estimate, ground truth of its object in its image): scene_id, im_id,
-        obj_id, est_id, gt_id, score, then per type: vsd_0 .. vsd_9 (one per tau of VSD_TAUS), mssd / mspd / add / adi (mm,
-        px) and mssd_sym / mspd_sym (index of the minimising symmetry, -1 where the error was not computed)."""
+        obj_id, est_id, gt_id, score, then per type: vsd_0 .. vsd_9 (one per tau of VSD_TAUS), mssd / mspd / add / adi /
+        ad (mm), mspd / proj (px), cus, re (degrees), te (mm), and mssd_sym / mspd_sym (index of the minimising symmetry, -1
+        where the error was not computed).  rete writes the re and te columns.  The toolkit's gating: ad / add / adi / mssd
+        are inf where the centres are a diameter or more apart, vsd / cus 1.0 where the projections of the bounding
+        spheres do not overlap; mspd, proj, re and te are always computed."""
         import pandas as pd
 
+        types = list(dict.fromkeys(types))
+        for t in types:
+            if t not in ERROR_TYPES:
+                raise ValueError(f"unknown error type {t!r} (one of {', '.join(ERROR_TYPES)})")
         sel = select_estimates(self.split, normalize_results(results))
         rows = self._pairs(sel)
         df = pd.DataFrame({k: [r[k] for r in rows] for k in ("scene_id", "im_id", "obj_id", "est_id", "gt_id", "score")})
+        rendered = self._vsd(sel, rows, [t for t in types if t in ("vsd", "cus")]) if {"vsd", "cus"} & set(types) else {}
+        pose_types = [t for t in ("proj", "re", "te") if t in types or (t != "proj" and "rete" in types)]
+        posed = self._pose(pose_types, sel, rows) if pose_types else {}
         for t in types:
             if t == "vsd":
-                v = self._vsd(sel, rows)
+                v = rendered["vsd"]
                 for k in range(v.shape[1]):
                     df[f"vsd_{k}"] = v[:, k]
+            elif t == "cus":
+                df["cus"] = rendered["cus"]
             elif t in KINDS:
                 e, a = self._point(t, sel, rows)
                 df[t] = e
                 if t in ("mssd", "mspd"):
                     df[f"{t}_sym"] = a
-            else:
-                raise ValueError(f"unknown error type {t!r}")
+            elif t == "ad":
+                df["ad"] = self._ad(sel, rows)
+            elif t == "rete":
+                for c in ("re", "te"):
+                    if c not in df:
+                        df[c] = posed[c]
+            elif t not in df:  # proj, re, te
+                df[t] = posed[t]
         return df
 
-    def evaluate(self, results, errors_out: Optional[Union[str, Path]] = None) -> dict:
+    def evaluate(self, results, errors_out: Optional[Union[str, Path]] = None, types: Iterable[str] = BOP19_TYPES,
+                 thresholds: Optional[Dict[str, Sequence[float]]] = None) -> dict:
+        """score_errors of `errors(results, types)`.  The bop19 keys are those of the bop19 types asked for; each other type
+        gets the toolkit's score dict under its name, at LOCALIZATION_THRESHOLDS or the `thresholds` given per type (te in
+        mm).  With `ad`, `symmetric_obj_ids` records the objects it scored with ADI."""
+        types = list(dict.fromkeys(types))
+        ths = resolve_thresholds(thresholds)
         ests = normalize_results(results)
-        df = self.errors(ests)
+        df = self.errors(ests, types)
         if errors_out is not None:
             Path(errors_out).mkdir(parents=True, exist_ok=True)
             df.to_csv(Path(errors_out) / "errors.csv", index=False)
-        return score_errors(self.split, df, ests)
+        scores = score_errors(self.split, df, ests, types, ths)
+        if "ad" in types:
+            scores["symmetric_obj_ids"] = list(self.symmetric_obj_ids)
+        return scores
+
+
+def parse_error_types(text: str) -> List[str]:
+    types = [t.strip() for t in text.split(",") if t.strip()]
+    for t in types:
+        if t not in ERROR_TYPES:
+            raise argparse.ArgumentTypeError(f"unknown error type {t!r} (one of {', '.join(ERROR_TYPES)})")
+    return types
+
+
+def parse_correct_th(text: str) -> Tuple[str, List[float]]:
+    """`te=50` or `rete=5,10` -> (type, thresholds)."""
+    t, sep, v = text.partition("=")
+    if not sep or t.strip() not in LOCALIZATION_THRESHOLDS:
+        raise argparse.ArgumentTypeError(f"expected <type>=<threshold>[,<threshold>] with a type among "
+                                         f"{', '.join(LOCALIZATION_THRESHOLDS)}, got {text!r}")
+    try:
+        return t.strip(), [float(x) for x in v.split(",")]
+    except ValueError as e:
+        raise argparse.ArgumentTypeError(str(e)) from None
+
+
+def add_error_type_arguments(ap: argparse.ArgumentParser, prefix: str = "") -> None:
+    """--[prefix]error-types, --correct-th, --symmetric-obj-ids (shared with prediction_runner --evaluate)."""
+    ap.add_argument(f"--{prefix}error-types", type=parse_error_types, default=None,
+                    help="comma-separated error types to score instead of the bop19 ones (vsd, mssd, mspd): any of "
+                         f"{', '.join(ERROR_TYPES)}; each type other than the bop19 ones gets the BOP toolkit's score dict "
+                         "(recall, per-object and per-scene recalls)")
+    ap.add_argument("--correct-th", type=parse_correct_th, action="append", default=[], metavar="TYPE=TH[,TH]",
+                    help="correctness threshold(s) of one error type, repeatable (the toolkit's --correct_th_<type>); "
+                         "defaults: " + ", ".join(f"{t}={','.join(f'{x:g}' for x in v)}"
+                                                  for t, v in LOCALIZATION_THRESHOLDS.items())
+                         + ". ad/add/adi are fractions of the diameter, proj px, re degrees; te is in mm, the unit of "
+                           "its errors, although the toolkit labels it cm")
+    ap.add_argument("--symmetric-obj-ids", default=None,
+                    help="comma-separated objects that `ad` scores with ADI (default: those with symmetries in "
+                         "models_info)")
+
+
+def error_type_options(args: argparse.Namespace, prefix: str = "") -> dict:
+    """BopEvaluator keyword arguments and evaluate() keyword arguments from add_error_type_arguments' options."""
+    types = getattr(args, f"{prefix}error_types".replace("-", "_"))
+    sym = args.symmetric_obj_ids
+    return dict(types=list(types) if types else list(BOP19_TYPES), thresholds=dict(args.correct_th),
+                symmetric_obj_ids=[int(o) for o in sym.split(",") if o.strip()] if sym is not None else None)
 
 
 def main(argv: Optional[Sequence[str]] = None) -> dict:
-    ap = argparse.ArgumentParser(description="BOP 2019 average recall (VSD, MSSD, MSPD) of a bop19 results CSV")
+    ap = argparse.ArgumentParser(description="BOP 2019 average recall (VSD, MSSD, MSPD) of a bop19 results CSV, and the "
+                                             "BOP toolkit's other pose-error scores (--error-types)")
     ap.add_argument("dataset_dir")
     ap.add_argument("results_csv")
     ap.add_argument("--split", default="test")
     ap.add_argument("--errors-out", default=None, help="directory for the per-pair error table (errors.csv)")
+    add_error_type_arguments(ap)
     args = ap.parse_args(argv)
-    scores = BopEvaluator(args.dataset_dir, args.split).evaluate(args.results_csv, errors_out=args.errors_out)
+    opt = error_type_options(args)
+    ev = BopEvaluator(args.dataset_dir, args.split, symmetric_obj_ids=opt["symmetric_obj_ids"])
+    scores = ev.evaluate(args.results_csv, errors_out=args.errors_out, types=opt["types"], thresholds=opt["thresholds"])
     print(json.dumps(scores))
     return scores
 

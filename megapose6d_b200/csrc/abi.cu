@@ -655,6 +655,44 @@ int mpx_bop_gt_info(int n_gt, int h, int w, const uint16_t* d_depth_test, int n_
                      d_bbox, d_mask, d_mask_visib, static_cast<cudaStream_t>(stream));
 }
 
+int mpx_bop_cus(int n_pairs, int h, int w, const float* d_depth_est, int n_est, const float* d_depth_gt, int n_gt,
+                const int32_t* d_est_idx, const int32_t* d_gt_idx, int64_t* d_counts, double* d_err, void* stream) {
+  MPX_REQUIRE(n_pairs >= 0, "mpx_bop_cus: n_pairs=%d < 0", n_pairs);
+  if (n_pairs == 0) return MPX_OK;
+  MPX_REQUIRE(h > 0 && w > 0 && static_cast<long long>(h) * w < (1ll << 31), "mpx_bop_cus: bad image size %dx%d", h, w);
+  MPX_REQUIRE(n_est > 0 && n_gt > 0, "mpx_bop_cus: n_est=%d n_gt=%d", n_est, n_gt);
+  MPX_DEVICE(d_depth_est);
+  MPX_DEVICE(d_depth_gt);
+  MPX_DEVICE(d_est_idx);
+  MPX_DEVICE(d_gt_idx);
+  MPX_DEVICE(d_counts);
+  MPX_DEVICE(d_err);
+  return bop_cus(n_pairs, h, w, d_depth_est, n_est, d_depth_gt, n_gt, d_est_idx, d_gt_idx, d_counts, d_err,
+                 static_cast<cudaStream_t>(stream));
+}
+
+int mpx_bop_pose_errors(int n_pairs, int n_models, const double* d_pts, const int64_t* d_pt_offsets, long long n_pts_total,
+                        const int32_t* d_model_idx, const double* d_pose_est, const double* d_pose_gt, const double* d_K,
+                        double* d_proj, double* d_re, double* d_te, void* stream) {
+  MPX_REQUIRE(n_pairs >= 0, "mpx_bop_pose_errors: n_pairs=%d < 0", n_pairs);
+  if (n_pairs == 0) return MPX_OK;
+  MPX_DEVICE(d_pose_est);
+  MPX_DEVICE(d_pose_gt);
+  MPX_DEVICE_OR_NULL(d_re);
+  MPX_DEVICE_OR_NULL(d_te);
+  if (d_proj) {
+    MPX_REQUIRE(n_models >= 1 && n_pts_total >= 0, "mpx_bop_pose_errors: n_models=%d n_pts_total=%lld", n_models,
+                n_pts_total);
+    MPX_DEVICE(d_proj);
+    MPX_DEVICE(d_pts);
+    MPX_DEVICE(d_pt_offsets);
+    MPX_DEVICE(d_model_idx);
+    MPX_DEVICE(d_K);
+  }
+  return bop_pose_errors(n_pairs, n_models, d_pts, d_pt_offsets, n_pts_total, d_model_idx, d_pose_est, d_pose_gt, d_K,
+                         d_proj, d_re, d_te, static_cast<cudaStream_t>(stream));
+}
+
 // ---- detector: ResNet-50 FPN + RPN head ----
 struct mpx_fpn {
   Fpn* fpn;

@@ -11,6 +11,9 @@
 // Point errors: one CTA per pair.  MSSD / MSPD take the max over the model points of each (pair, symmetry) and the min over
 // the symmetries (first minimum wins, as Python's min); ADD is the mean point distance; ADI the mean nearest-neighbour
 // distance, by brute force over shared-memory tiles of the estimate's points, all in float64.
+//
+// CUS counts the two silhouettes of the VSD layout's renders as the VSD count kernel counts; PROJ / RE / TE
+// (mpx_bop_pose_errors) take one CTA per pair, PROJ with ADD's block sum.
 #include "mpx_common.cuh"
 #include "../../include/mpx.h"
 
@@ -162,6 +165,76 @@ int bop_vsd(int n_pairs, int h, int w, const uint16_t* test, int n_img, const fl
   }
   bop_vsd_finish_kernel<<<(n_pairs + 127) / 128, 128, 0, stream>>>(n_pairs, n_taus, est_idx, gt_idx, img_idx, n_est, n_gt,
                                                                    n_img, cnt, err);
+  MPX_CHECK_CUDA(cudaGetLastError());
+  ++g_launches;
+  return MPX_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// CUS: complement over union of the two silhouettes (pose_error.cus), on the VSD kernel's render-sharing layout
+// ---------------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool cus_pair_valid(int p, const int* est_idx, const int* gt_idx, int n_est, int n_gt) {
+  const int e = est_idx[p], g = gt_idx[p];
+  return e >= 0 && e < n_est && g >= 0 && g < n_gt;
+}
+
+// counts[p] = {intersection, union}, zeroed before the launch
+__global__ void __launch_bounds__(kVsdThreads) bop_cus_count_kernel(
+    int pair0, int hw, const float* __restrict__ dest, int n_est, const float* __restrict__ dgt, int n_gt,
+    const int* __restrict__ est_idx, const int* __restrict__ gt_idx, unsigned long long* __restrict__ counts) {
+  const int p = pair0 + blockIdx.y;
+  if (!cus_pair_valid(p, est_idx, gt_idx, n_est, n_gt)) return;
+  const float* e_im = dest + static_cast<size_t>(est_idx[p]) * hw;
+  const float* g_im = dgt + static_cast<size_t>(gt_idx[p]) * hw;
+  unsigned n_inter = 0, n_union = 0;
+  for (int px = blockIdx.x * blockDim.x + threadIdx.x; px < hw; px += gridDim.x * blockDim.x) {
+    // fp32(metres * 1000) > 0 exactly when metres > 0: the mask of the toolkit's depth in mm
+    const bool me = e_im[px] > 0.f, mg = g_im[px] > 0.f;
+    n_inter += me && mg;
+    n_union += me || mg;
+  }
+  __shared__ unsigned long long part[kVsdThreads / 32][2];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned long long v = warp_sum_u64(n_inter);
+  if (lane == 0) part[warp][0] = v;
+  v = warp_sum_u64(n_union);
+  if (lane == 0) part[warp][1] = v;
+  __syncthreads();
+  if (threadIdx.x < 2) {
+    unsigned long long s = 0;
+    for (int i = 0; i < kVsdThreads / 32; ++i) s += part[i][threadIdx.x];
+    if (s) atomicAdd(counts + 2 * static_cast<size_t>(p) + threadIdx.x, s);
+  }
+}
+
+// 1.0 - inter / float(union) in float64, as the toolkit writes it; 1.0 for an empty union, NaN for out-of-range indices
+__global__ void bop_cus_finish_kernel(int n_pairs, const int* __restrict__ est_idx, const int* __restrict__ gt_idx,
+                                      int n_est, int n_gt, const unsigned long long* __restrict__ counts,
+                                      double* __restrict__ err) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n_pairs) return;
+  const unsigned long long inter = counts[2 * static_cast<size_t>(p)], uni = counts[2 * static_cast<size_t>(p) + 1];
+  double e;
+  if (!cus_pair_valid(p, est_idx, gt_idx, n_est, n_gt)) e = __longlong_as_double(0x7ff8000000000000ll);
+  else if (uni == 0) e = 1.0;
+  else e = __dadd_rn(1.0, -__ddiv_rn(static_cast<double>(inter), static_cast<double>(uni)));
+  err[p] = e;
+}
+
+int bop_cus(int n_pairs, int h, int w, const float* dest, int n_est, const float* dgt, int n_gt, const int* est_idx,
+            const int* gt_idx, int64_t* counts, double* err, cudaStream_t stream) {
+  if (n_pairs == 0) return MPX_OK;
+  const int hw = h * w;
+  MPX_CHECK_CUDA(cudaMemsetAsync(counts, 0, sizeof(int64_t) * 2 * static_cast<size_t>(n_pairs), stream));
+  const int bx = (hw + kVsdThreads * kVsdPixelsPerThread - 1) / (kVsdThreads * kVsdPixelsPerThread);
+  auto* cnt = reinterpret_cast<unsigned long long*>(counts);
+  for (int p0 = 0; p0 < n_pairs; p0 += 65535) {  // gridDim.y limit
+    const int np = n_pairs - p0 < 65535 ? n_pairs - p0 : 65535;
+    bop_cus_count_kernel<<<dim3(bx, np), kVsdThreads, 0, stream>>>(p0, hw, dest, n_est, dgt, n_gt, est_idx, gt_idx, cnt);
+    MPX_CHECK_CUDA(cudaGetLastError());
+    ++g_launches;
+  }
+  bop_cus_finish_kernel<<<(n_pairs + 127) / 128, 128, 0, stream>>>(n_pairs, est_idx, gt_idx, n_est, n_gt, cnt, err);
   MPX_CHECK_CUDA(cudaGetLastError());
   ++g_launches;
   return MPX_OK;
@@ -524,6 +597,103 @@ int bop_point_errors(int kind, int n_pairs, int n_models, const double* pts, con
                                        : bop_point_kernel<MPX_BOP_ADI>;
   kernel<<<n_pairs, kPointThreads, 0, stream>>>(n_models, pts, pt_off, n_pts_total, syms, sym_off, n_syms_total, model_idx,
                                                 pose_est, pose_gt, K, err, sym_argmin);
+  MPX_CHECK_CUDA(cudaGetLastError());
+  ++g_launches;
+  return MPX_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// PROJ, RE, TE (pose_error.proj, re, te)
+// ---------------------------------------------------------------------------------------------------------------------
+// pose_error.re: acos of 0.5 (trace(R_est inv(R_gt)) - 1), clipped to [-1, 1], in degrees.  The inverse is the true one
+// (adjugate over determinant), not the transpose: rotations read from text are orthonormal only to their printed digits.
+__device__ double rotation_error_deg(const double* e, const double* g) {
+  const double c00 = __dadd_rn(__dmul_rn(g[4], g[8]), -__dmul_rn(g[5], g[7]));
+  const double c01 = __dadd_rn(__dmul_rn(g[5], g[6]), -__dmul_rn(g[3], g[8]));
+  const double c02 = __dadd_rn(__dmul_rn(g[3], g[7]), -__dmul_rn(g[4], g[6]));
+  const double det = __dadd_rn(__dadd_rn(__dmul_rn(g[0], c00), __dmul_rn(g[1], c01)), __dmul_rn(g[2], c02));
+  double inv[9];  // row-major inv(R_gt)
+  inv[0] = __ddiv_rn(c00, det);
+  inv[3] = __ddiv_rn(c01, det);
+  inv[6] = __ddiv_rn(c02, det);
+  inv[1] = __ddiv_rn(__dadd_rn(__dmul_rn(g[2], g[7]), -__dmul_rn(g[1], g[8])), det);
+  inv[2] = __ddiv_rn(__dadd_rn(__dmul_rn(g[1], g[5]), -__dmul_rn(g[2], g[4])), det);
+  inv[4] = __ddiv_rn(__dadd_rn(__dmul_rn(g[0], g[8]), -__dmul_rn(g[2], g[6])), det);
+  inv[5] = __ddiv_rn(__dadd_rn(__dmul_rn(g[2], g[3]), -__dmul_rn(g[0], g[5])), det);
+  inv[7] = __ddiv_rn(__dadd_rn(__dmul_rn(g[1], g[6]), -__dmul_rn(g[0], g[7])), det);
+  inv[8] = __ddiv_rn(__dadd_rn(__dmul_rn(g[0], g[4]), -__dmul_rn(g[1], g[3])), det);
+  double tr = 0.0;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const double d = __dadd_rn(__dadd_rn(__dmul_rn(e[3 * i], inv[i]), __dmul_rn(e[3 * i + 1], inv[3 + i])),
+                               __dmul_rn(e[3 * i + 2], inv[6 + i]));
+    tr = i ? __dadd_rn(tr, d) : d;
+  }
+  const double c = fmin(1.0, fmax(-1.0, __dmul_rn(0.5, __dadd_rn(tr, -1.0))));
+  return __ddiv_rn(__dmul_rn(180.0, acos(c)), 3.141592653589793);
+}
+
+// pose_error.te: |t_gt - t_est| (mm)
+__device__ double translation_error(const double* e, const double* g) {
+  const double dx = __dadd_rn(g[9], -e[9]), dy = __dadd_rn(g[10], -e[10]), dz = __dadd_rn(g[11], -e[11]);
+  return __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)));
+}
+
+// One CTA per pair.  Thread 0 writes RE / TE; with PROJ the CTA projects the model's points under both poses (P = K [R|t]
+// formed first, as misc.project_pts) and sums the distances in ADD's fixed-order block reduction.
+__global__ void __launch_bounds__(kPointThreads) bop_pose_kernel(
+    int n_models, const double* __restrict__ pts, const int64_t* __restrict__ pt_off, long long n_pts_total,
+    const int* __restrict__ model_idx, const double* __restrict__ pose_est, const double* __restrict__ pose_gt,
+    const double* __restrict__ K, double* __restrict__ proj, double* __restrict__ re, double* __restrict__ te) {
+  const int p = blockIdx.x;
+  const double* pe = pose_est + 12 * p;
+  const double* pg = pose_gt + 12 * p;
+  if (threadIdx.x == 0) {
+    if (re) re[p] = rotation_error_deg(pe, pg);
+    if (te) te[p] = translation_error(pe, pg);
+  }
+  if (!proj) return;
+  __shared__ Rt est, gt;
+  __shared__ double P_est[12], P_gt[12];
+  __shared__ double red[kPointThreads / 32];
+  const int m = model_idx[p];
+  long long p0 = 0, p1 = 0;
+  if (m >= 0 && m < n_models) {
+    p0 = max(0ll, min(static_cast<long long>(pt_off[m]), n_pts_total));
+    p1 = max(p0, min(static_cast<long long>(pt_off[m + 1]), n_pts_total));
+  }
+  if (p1 == p0) {
+    if (threadIdx.x == 0) proj[p] = __longlong_as_double(0x7ff8000000000000ll);
+    return;
+  }
+  if (threadIdx.x < 12) (threadIdx.x < 9 ? est.R[threadIdx.x] : est.t[threadIdx.x - 9]) = pe[threadIdx.x];
+  else if (threadIdx.x < 24) (threadIdx.x < 21 ? gt.R[threadIdx.x - 12] : gt.t[threadIdx.x - 21]) = pg[threadIdx.x - 12];
+  __syncthreads();
+  if (threadIdx.x == 0) make_P(K + 9 * p, est, P_est);
+  else if (threadIdx.x == 32) make_P(K + 9 * p, gt, P_gt);
+  __syncthreads();
+  const long long n = p1 - p0;
+  const double* P = pts + 3 * p0;
+  double sum = 0.0;
+  for (long long i = threadIdx.x; i < n; i += kPointThreads) {
+    const double x = P[3 * i], y = P[3 * i + 1], z = P[3 * i + 2];
+    double eu, ev, gu, gv;
+    project(P_est, x, y, z, eu, ev);
+    project(P_gt, x, y, z, gu, gv);
+    const double du = eu - gu, dv = ev - gv;
+    sum += sqrt(du * du + dv * dv);
+  }
+  const double total = block_reduce<false>(sum, red);
+  if (threadIdx.x == 0) proj[p] = total / static_cast<double>(n);
+}
+
+int bop_pose_errors(int n_pairs, int n_models, const double* pts, const int64_t* pt_off, long long n_pts_total,
+                    const int* model_idx, const double* pose_est, const double* pose_gt, const double* K, double* proj,
+                    double* re, double* te, cudaStream_t stream) {
+  if (n_pairs == 0 || (!proj && !re && !te)) return MPX_OK;
+  // without PROJ one warp per pair is enough
+  bop_pose_kernel<<<n_pairs, proj ? kPointThreads : 32, 0, stream>>>(n_models, pts, pt_off, n_pts_total, model_idx,
+                                                                     pose_est, pose_gt, K, proj, re, te);
   MPX_CHECK_CUDA(cudaGetLastError());
   ++g_launches;
   return MPX_OK;

@@ -316,6 +316,11 @@ int bop_point_errors(int kind, int n_pairs, int n_models, const double* pts, con
 int bop_gt_info(int n_gt, int h, int w, const uint16_t* test, int n_img, const float* depth_scale, const double* K,
                 const float* large, const int* img_idx, float delta, int64_t* counts, int* bbox, uint8_t* mask,
                 uint8_t* mask_visib, cudaStream_t stream);
+int bop_cus(int n_pairs, int h, int w, const float* dest, int n_est, const float* dgt, int n_gt, const int* est_idx,
+            const int* gt_idx, int64_t* counts, double* err, cudaStream_t stream);
+int bop_pose_errors(int n_pairs, int n_models, const double* pts, const int64_t* pt_off, long long n_pts_total,
+                    const int* model_idx, const double* pose_est, const double* pose_gt, const double* K, double* proj,
+                    double* re, double* te, cudaStream_t stream);
 
 
 // teaser.cu

@@ -475,8 +475,8 @@ def main(argv: Optional[List[str]] = None) -> None:
     python -m megapose6d_b200.prediction_runner --bop-dataset <dir> [--split test] [--label-format "{label}"] [--evaluate]
     --model <name> --save-dir <dir>
     The bop19 target frames of a BOP split (bop_dataset.keep_bop19(BOPDataset(...))) with the meshes of <dir>/models and the
-    ground truth as detections; `--evaluate` scores the 'refiner/final' CSV with bop_eval.BopEvaluator on rank 0, prints
-    the scores as one JSON line and saves them as <save-dir>/bop19_scores.json.
+    ground truth as detections; `--evaluate` scores the 'refiner/final' CSV with bop_eval.BopEvaluator on rank 0
+    (`--eval-error-types`, `--correct-th`, `--symmetric-obj-ids` as bop_eval's CLI), prints the scores as one JSON line and saves them as <save-dir>/bop19_scores.json.
     Under torchrun the frames are sharded over the ranks (one process per GPU) and rank 0 writes the results."""
     import argparse
     import json
@@ -492,6 +492,9 @@ def main(argv: Optional[List[str]] = None) -> None:
     parser.add_argument("--label-format", default="{label}", help="object labels of --bop-dataset (the reference's "
                         "label_format, e.g. 'ycbv-{label}')")
     parser.add_argument("--evaluate", action="store_true", help="BOP 2019 scores of the predictions on --bop-dataset")
+    from .bop_eval import add_error_type_arguments
+
+    add_error_type_arguments(parser, prefix="eval-")  # --eval-error-types, --correct-th, --symmetric-obj-ids
     parser.add_argument("--model", type=str, default="megapose-1.0-RGB-multi-hypothesis", choices=sorted(NAMED_MODELS))
     parser.add_argument("--models-root", type=Path, default=None)
     parser.add_argument("--meshes-from", type=Path, default=None)
@@ -552,10 +555,12 @@ def main(argv: Optional[List[str]] = None) -> None:
         n = len(out["results"]["predictions"]["final"])
         print(f"wrote {n} pose(s) of {len(scene_ds)} frame(s) to {out['save_dir']}")
         if args.evaluate:
-            from .bop_eval import BopEvaluator
+            from .bop_eval import BopEvaluator, error_type_options
 
             csv = out["save_dir"] / "bop_refiner_final.csv"
-            scores = BopEvaluator(args.bop_dataset, args.split).evaluate(csv if csv.exists() else [])
+            opt = error_type_options(args, prefix="eval-")
+            scores = BopEvaluator(args.bop_dataset, args.split, symmetric_obj_ids=opt["symmetric_obj_ids"]).evaluate(
+                csv if csv.exists() else [], types=opt["types"], thresholds=opt["thresholds"])
             (out["save_dir"] / "bop19_scores.json").write_text(json.dumps(scores))
             print(json.dumps(scores))
     if dist.is_initialized():

@@ -1,4 +1,5 @@
-"""Time the BOP 2019 evaluator on the device against oracle/bop_ref.py on the host cores, per error type.
+"""Time the BOP evaluator on the device against the host oracle (oracle/bop_ref.py, oracle/bop_other_ref.py) on the host
+cores, per error type: the bop19 ones (vsd, mssd, mspd) and the toolkit's others (ad, add, adi, cus, proj, re, te, rete).
 
 The split is YCB-V-sized: the 21 procedural objects of `workloads.scenes.ycbv_scene` as models_eval (mm), 640x480 images
 with all 21 objects each (written by workloads/bop_split.py through the device scene renderer), estimates = ground truth
@@ -25,9 +26,11 @@ from megapose6d_b200 import bop_eval  # noqa: E402
 from megapose6d_b200.meshes import TriMesh  # noqa: E402
 from megapose6d_b200.object_dataset import RigidObject, RigidObjectDataset  # noqa: E402
 from megapose6d_b200.scene_renderer import Panda3dSceneRenderer  # noqa: E402
-from oracle import bop_ref, pipeline_ref  # noqa: E402
+from oracle import bop_other_ref, bop_ref, pipeline_ref  # noqa: E402
 from workloads import bop_split  # noqa: E402
 from workloads.scenes import ycbv_scene  # noqa: E402
+
+OTHER_TYPES = ("ad", "add", "adi", "cus", "proj", "re", "te", "rete")
 
 
 def gpu_info() -> dict:
@@ -91,7 +94,7 @@ def main() -> None:
         split_sub = bop_eval.BopSplit(ev.split.root, ev.split.split, ev.split.models_info, ev.split.models,
                                       [t for t in ev.split.targets if t["im_id"] < args.oracle_images],
                                       ev.split.scene_camera, ev.split.scene_gt, ev.split.scene_gt_info)
-        for t in ("vsd", "mssd", "mspd"):
+        for t in ("vsd", "mssd", "mspd") + OTHER_TYPES:
             ev.errors(ests_n, types=(t,))  # warm-up: mesh upload, module load
             torch.cuda.synchronize()
             t0 = time.perf_counter()
@@ -99,7 +102,10 @@ def main() -> None:
             torch.cuda.synchronize()
             dev_s = time.perf_counter() - t0
             t0 = time.perf_counter()
-            rows = bop_ref.calc_errors(split_sub, sub, host_render, types=(t,))
+            if t in OTHER_TYPES:
+                rows = bop_other_ref.calc_other_errors(split_sub, sub, host_render, (t,), ev.symmetric_obj_ids)
+            else:
+                rows = bop_ref.calc_errors(split_sub, sub, host_render, types=(t,))
             host_s = time.perf_counter() - t0
             dev_per_pair = dev_s / len(df)
             host_per_pair = host_s / max(1, len(rows))
