@@ -1458,14 +1458,19 @@ int raster_launch(const MeshDb* db, const int32_t* label_idx, const float* TCO, 
       }
     }
   }
+  // CTA b of the untiled kernel uses visibility buffer b of the workspace, which holds 2 x sm_count() of them, and vertex
+  // cache slot b of the mesh database, which holds db->slots (2 x sm_count() when it was created).  mpx_set_sm_limit can
+  // change sm_count() after the database exists, so the grid takes the smaller of the two; the persistent loop covers
+  // every (view, strip) item with any grid size.
+  const int slots = db->slots < 2 * sm_count() ? db->slots : 2 * sm_count();
   int strips = 1;
-  if (n_views < db->slots) {
-    strips = db->slots / n_views;
+  if (n_views < slots) {
+    strips = slots / n_views;
     if (strips > 16) strips = 16;
     if (strips > h) strips = h;
   }
   const long long items = static_cast<long long>(n_views) * strips;
-  const int grid = items < db->slots ? static_cast<int>(items) : db->slots;
+  const int grid = items < slots ? static_cast<int>(items) : slots;
   if (db->tex_info != nullptr)
     raster_kernel<true><<<grid, kRasterThreads, 0, stream>>>(*db, label_idx, TCO, K, n_views, h, w, flags, out,
                                                              reinterpret_cast<unsigned long long*>(workspace), strips);
