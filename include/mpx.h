@@ -375,6 +375,60 @@ int mpx_mask_paste(const float* d_logits, const int64_t* d_labels, const float* 
                    int m, int n_images, const int32_t* h_counts, const int32_t* h_sizes, float* d_boxes_out,
                    float* const* h_masks, void* stream);
 
+/* ---- detector: RoI heads ---------------------------------------------------------------------------
+ * The box and mask branches of torchvision's RoIHeads (eval) for n_images images, RoIs given per image (the detections of
+ * image 0 first).  Every matrix product runs on the wgmma convolution (act16 operands and activations, fp32
+ * accumulation, one rounding per layer after bias and ReLU); the pooled features are rounded once to act16.
+ *
+ * Pooling (MultiScaleRoIAlign on the FPN levels '0'..'3', aligned=False): each RoI goes to the level of torchvision's
+ * LevelMapper, floor(canonical_level + log2(sqrt(area) / canonical_scale) + 1e-6) clamped to the four levels, each
+ * operation rounded to fp32 on its own as ATen rounds it; roi_align then uses that level's spatial scale and
+ * sampling_ratio x sampling_ratio samples per bin, in the expressions of torchvision's CUDA kernel.
+ *   h_features  HOST array of 4 DEVICE pointers, fp32 NCHW [n_images, 256, h >> (l + 2), w >> (l + 2)] (mpx_fpn_forward's
+ *               levels '0'..'3' of a padded h x w batch, h and w multiples of 32)
+ *   h_scales    HOST [4] fp32: 2^-k, 2^-(k+1), 2^-(k+2), 2^-(k+3) (Mask R-CNN: 1/4 .. 1/32)
+ *   d_boxes     [n_rois, 4] fp32 (x0, y0, x1, y1) in the padded batch's pixels; h_counts HOST [n_images] RoIs per image
+ * sampling_ratio 1..16, n_images 1..64, at most 1,000,000 RoIs in all (the mask branch: n_rois * 4 * mask_pool^2 < 2^31).
+ * Zero RoIs launch nothing.  A box of negative area gets torchvision's level for it, 0 - k, which pools to zeros;
+ * d_levels reports it as such.
+ *
+ * mpx_roi_heads_create: h_conv_w / h_conv_b are HOST arrays of 9 DEVICE pointers, act16 [C_out, R*S*C_in] with
+ * k = (r, s, c) and fp32 [C_out], in execution order:
+ *   0  box_head.fc6 as a 7x7 convolution 256 -> hidden: weight (o, y, x, c) = fc6.weight[o, c * 49 + y * 7 + x]
+ *   1  box_head.fc7 as a 1x1 convolution hidden -> hidden
+ *   2  box_predictor cls_score | bbox_pred as one 1x1 hidden -> 5 x n_classes rounded up to 64, the rest zero
+ *   3..6  mask_head's four 3x3 convolutions 256 -> 256 (ReLU)
+ *   7  mask_predictor.conv5_mask (ConvTranspose2d 256 -> 256, 2x2, stride 2) as a 1x1 convolution 256 -> 1024: row
+ *      (dy * 2 + dx) * 256 + o is weight[:, o, dy, dx], bias[o]
+ *   8  mask_predictor.mask_fcn_logits as a 1x1 convolution 256 -> n_classes rounded up to 64, the rest zero
+ * n_classes 1..409, hidden a multiple of 64 in 64..2048.  The handle keeps the pointers; the tensors must outlive it. */
+typedef struct mpx_roi_heads mpx_roi_heads;
+int mpx_roi_heads_create(const void* const* h_conv_w, const float* const* h_conv_b, int n_convs, int n_classes,
+                         int hidden, mpx_roi_heads** out);
+int mpx_roi_heads_destroy(mpx_roi_heads* heads);
+/* bytes of workspace for one box call over n_box_rois RoIs and one mask call over n_mask_rois RoIs pooled to
+ * mask_pool x mask_pool (0 for arguments the calls refuse) */
+size_t mpx_roi_heads_workspace_bytes(const mpx_roi_heads* heads, int n_box_rois, int n_mask_rois, int mask_pool);
+/* The pooling step alone: d_pooled [n_rois, out_size, out_size, 256] fp32 (NHWC, before the act16 rounding), d_levels
+ * [n_rois] int32 the level index 0..3 of each RoI (may be NULL).  out_size 1..32. */
+int mpx_roi_pool(const float* const* h_features, int n_images, int h, int w, const float* h_scales, int canonical_scale,
+                 int canonical_level, int sampling_ratio, const float* d_boxes, const int32_t* h_counts, int out_size,
+                 float* d_pooled, int32_t* d_levels, void* stream);
+/* Box branch: 7x7 pool, fc6 + ReLU, fc7 + ReLU, predictor.  d_class_logits [n_rois, n_classes] and d_box_regression
+ * [n_rois, 4 n_classes] fp32, exact conversions of the act16 predictor outputs. */
+int mpx_roi_box_forward(const mpx_roi_heads* heads, const float* const* h_features, int n_images, int h, int w,
+                        const float* h_scales, int canonical_scale, int canonical_level, int sampling_ratio,
+                        const float* d_boxes, const int32_t* h_counts, float* d_class_logits, float* d_box_regression,
+                        void* d_workspace, size_t workspace_bytes, void* stream);
+/* Mask branch: mask_pool x mask_pool pool (1..32), the four 3x3 convolutions + ReLU, the deconvolution + ReLU, the
+ * logits.  d_mask_logits [n_rois, n_classes, 2 mask_pool, 2 mask_pool] fp32, the layout mpx_mask_paste reads.
+ * Both branches refuse, before any launch: a NULL handle, bad sizes, scales or counts, NULL or non-device pointers, a
+ * workspace smaller than mpx_roi_heads_workspace_bytes or not 256-byte aligned. */
+int mpx_roi_mask_forward(const mpx_roi_heads* heads, const float* const* h_features, int n_images, int h, int w,
+                         const float* h_scales, int canonical_scale, int canonical_level, int sampling_ratio,
+                         int mask_pool, const float* d_boxes, const int32_t* h_counts, float* d_mask_logits,
+                         void* d_workspace, size_t workspace_bytes, void* stream);
+
 /* ---- BOP 2019 pose errors ------------------------------------------------------------------------
  * The pose-error functions of the BOP toolkit (bop_toolkit_lib/pose_error.py: vsd, mssd, mspd, add, adi, cus, proj, re,
  * te), vendored by the

@@ -75,6 +75,17 @@ def _declare(lib: ctypes.CDLL) -> None:
     lib.mpx_fpn_forward.argtypes = [vp, vp, c_int, c_int, c_int, POINTER(vp), POINTER(vp), POINTER(vp), vp, c_size_t, vp]
     lib.mpx_mask_paste.argtypes = [vp, vp, vp, c_int, c_int, c_int, c_int, POINTER(ctypes.c_int32), POINTER(ctypes.c_int32),
                                    vp, POINTER(vp), vp]
+    i32p = POINTER(ctypes.c_int32)
+    lib.mpx_roi_heads_create.argtypes = [POINTER(vp), POINTER(vp), c_int, c_int, c_int, POINTER(vp)]
+    lib.mpx_roi_heads_destroy.argtypes = [vp]
+    lib.mpx_roi_heads_workspace_bytes.argtypes = [vp, c_int, c_int, c_int]
+    lib.mpx_roi_heads_workspace_bytes.restype = c_size_t
+    lib.mpx_roi_pool.argtypes = [POINTER(vp), c_int, c_int, c_int, POINTER(c_float), c_int, c_int, c_int, vp, i32p, c_int,
+                                 vp, vp, vp]
+    lib.mpx_roi_box_forward.argtypes = [vp, POINTER(vp), c_int, c_int, c_int, POINTER(c_float), c_int, c_int, c_int, vp,
+                                        i32p, vp, vp, vp, c_size_t, vp]
+    lib.mpx_roi_mask_forward.argtypes = [vp, POINTER(vp), c_int, c_int, c_int, POINTER(c_float), c_int, c_int, c_int, c_int,
+                                         vp, i32p, vp, vp, c_size_t, vp]
     lib.mpx_bop_vsd.argtypes = [c_int, c_int, c_int, vp, c_int, vp, vp, vp, c_int, vp, c_int, vp, vp, vp, vp, vp, c_int,
                                 c_float, vp, vp, vp]
     lib.mpx_bop_point_errors.argtypes = [c_int, c_int, c_int, vp, vp, ctypes.c_longlong, vp, vp, ctypes.c_longlong, vp, vp,
@@ -115,6 +126,8 @@ EXPORTS = [
     "mpx_net_input_bytes", "mpx_conv2d", "mpx_conv2d_splitk", "mpx_conv_set_mode", "mpx_maxpool3x3s2", "mpx_avgpool_linear",
     "mpx_net_create", "mpx_net_create_preact", "mpx_net_destroy", "mpx_net_set_graphs", "mpx_net_workspace_bytes", "mpx_net_forward",
     "mpx_fpn_create", "mpx_fpn_destroy", "mpx_fpn_workspace_bytes", "mpx_fpn_forward", "mpx_mask_paste",
+    "mpx_roi_heads_create", "mpx_roi_heads_destroy", "mpx_roi_heads_workspace_bytes", "mpx_roi_pool", "mpx_roi_box_forward",
+    "mpx_roi_mask_forward",
     "mpx_bop_vsd", "mpx_bop_point_errors", "mpx_bop_gt_info", "mpx_bop_cus", "mpx_bop_pose_errors",
     "mpx_teaser_points", "mpx_teaser_fps_workspace_bytes", "mpx_teaser_fps", "mpx_teaser_graph",
     "mpx_teaser_clique_workspace_bytes", "mpx_teaser_max_clique", "mpx_teaser_solve",

@@ -15,7 +15,7 @@ from pathlib import Path
 
 CSRC = Path(__file__).resolve().parent / "csrc"
 LIB_PATH = CSRC / "libmpx.so"
-SOURCES = ["abi.cu", "conv_wgmma.cu", "net.cu", "detector_net.cu", "raster.cu", "geom.cu", "crop.cu", "bop_eval.cu", "teaser.cu"]
+SOURCES = ["abi.cu", "conv_wgmma.cu", "net.cu", "detector_net.cu", "detector_heads.cu", "raster.cu", "geom.cu", "crop.cu", "bop_eval.cu", "teaser.cu"]
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
     *ARCH_FLAGS,

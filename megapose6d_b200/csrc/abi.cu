@@ -1,6 +1,7 @@
 // extern "C" surface of libmpx.so (declared in include/mpx.h). Thin argument validation + dispatch;
 // every entry point enqueues work on the caller's stream and returns without synchronising.
 #include <stdarg.h>
+#include <cmath>
 #include "mpx_common.cuh"
 #include "../../include/mpx.h"
 
@@ -780,6 +781,147 @@ int mpx_mask_paste(const float* d_logits, const int64_t* d_labels, const float* 
   }
   return mask_paste(d_logits, reinterpret_cast<const long long*>(d_labels), d_boxes, n_masks, n_classes, m, n_images,
                     h_counts, h_sizes, d_boxes_out, h_masks, static_cast<cudaStream_t>(stream));
+}
+
+// ---- detector: RoI heads ----
+struct mpx_roi_heads {
+  RoiHeads* heads;
+  int n_classes;
+};
+
+int mpx_roi_heads_create(const void* const* h_conv_w, const float* const* h_conv_b, int n_convs, int n_classes,
+                         int hidden, mpx_roi_heads** out) {
+  MPX_NOT_NULL(h_conv_w);
+  MPX_NOT_NULL(h_conv_b);
+  MPX_NOT_NULL(out);
+  MPX_REQUIRE(n_convs == kRoiHeadConvs, "mpx_roi_heads_create: expected %d conv tensors, got %d", kRoiHeadConvs, n_convs);
+  MPX_REQUIRE(n_classes >= 1 && roi_box_rows(n_classes) <= 2048,
+              "mpx_roi_heads_create: %d classes: need 1..409 (5 x classes rounded up to 64 at most 2048)", n_classes);
+  MPX_REQUIRE(hidden >= 64 && hidden <= 2048 && hidden % 64 == 0,
+              "mpx_roi_heads_create: representation size %d must be a multiple of 64 in 64..2048", hidden);
+  for (int i = 0; i < n_convs; ++i)
+    MPX_REQUIRE(is_device_ptr(h_conv_w[i]) && is_device_ptr(h_conv_b[i]),
+                "mpx_roi_heads_create: conv %d has a NULL or non-device tensor", i);
+  RoiHeads* heads = nullptr;
+  int rc = roi_heads_create(h_conv_w, h_conv_b, n_classes, hidden, &heads);
+  if (rc != MPX_OK) return rc;
+  *out = new mpx_roi_heads{heads, n_classes};
+  return MPX_OK;
+}
+
+int mpx_roi_heads_destroy(mpx_roi_heads* heads) {
+  if (heads) {
+    roi_heads_destroy(heads->heads);
+    delete heads;
+  }
+  return MPX_OK;
+}
+
+// The mask branch's largest convolution has n_rois * 4 * mask_pool^2 output pixels; conv_forward takes fewer than 2^31.
+static bool mask_rois_ok(long long n_rois, int mask_pool) {
+  return n_rois * 4 * mask_pool * mask_pool < (1ll << 31);
+}
+
+size_t mpx_roi_heads_workspace_bytes(const mpx_roi_heads* heads, int n_box_rois, int n_mask_rois, int mask_pool) {
+  if (heads == nullptr || n_box_rois < 0 || n_box_rois > kRoiMaxRois || n_mask_rois < 0 || mask_pool < 1 ||
+      mask_pool > kMaskMaxM / 2 || !mask_rois_ok(n_mask_rois, mask_pool))
+    return 0;
+  return roi_heads_workspace_bytes(heads->heads, n_box_rois, n_mask_rois, mask_pool);
+}
+
+// Checks shared by the pool and both branches; returns the RoI count through n_rois.
+static int roi_args_ok(const char* fn, const float* const* h_features, int n_images, int h, int w, const float* h_scales,
+                       int canonical_scale, int canonical_level, int sampling, const float* d_boxes,
+                       const int32_t* h_counts, long long* n_rois) {
+  MPX_REQUIRE(n_images >= 1 && n_images <= kMaskMaxImages, "%s: n_images=%d, must be 1..%d", fn, n_images, kMaskMaxImages);
+  MPX_REQUIRE(h >= 32 && w >= 32 && h % 32 == 0 && w % 32 == 0, "%s: batch %dx%d: need positive multiples of 32", fn, h,
+              w);
+  MPX_REQUIRE(h_features != nullptr && h_scales != nullptr && h_counts != nullptr,
+              "%s: h_features, h_scales and h_counts must not be NULL", fn);
+  const double k_min = -std::log2(static_cast<double>(h_scales[0]));
+  for (int l = 0; l < 4; ++l) {
+    MPX_REQUIRE(is_device_ptr(h_features[l]), "%s: feature level %d is NULL or not device memory", fn, l);
+    MPX_REQUIRE(k_min >= 0 && k_min <= 16 && k_min == std::round(k_min) && h_scales[l] == std::exp2(-(k_min + l)),
+                "%s: the scales must be 2^-k, 2^-(k+1), ... (got %g at level %d)", fn, h_scales[l], l);
+  }
+  MPX_REQUIRE(canonical_scale >= 1 && canonical_level >= 0 && canonical_level <= 16,
+              "%s: canonical scale %d / level %d", fn, canonical_scale, canonical_level);
+  MPX_REQUIRE(sampling >= 1 && sampling <= 16, "%s: sampling_ratio=%d, must be 1..16", fn, sampling);
+  long long total = 0;
+  for (int i = 0; i < n_images; ++i) {
+    MPX_REQUIRE(h_counts[i] >= 0, "%s: image %d has %d RoIs", fn, i, h_counts[i]);
+    total += h_counts[i];
+  }
+  MPX_REQUIRE(total <= kRoiMaxRois, "%s: %lld RoIs, at most %d", fn, total, kRoiMaxRois);
+  if (total > 0) MPX_REQUIRE(is_device_ptr(d_boxes), "%s: d_boxes is NULL or not device memory", fn);
+  *n_rois = total;
+  return MPX_OK;
+}
+
+int mpx_roi_pool(const float* const* h_features, int n_images, int h, int w, const float* h_scales, int canonical_scale,
+                 int canonical_level, int sampling, const float* d_boxes, const int32_t* h_counts, int out_size,
+                 float* d_pooled, int32_t* d_levels, void* stream) {
+  long long n = 0;
+  int rc = roi_args_ok(__func__, h_features, n_images, h, w, h_scales, canonical_scale, canonical_level, sampling, d_boxes,
+                       h_counts, &n);
+  if (rc != MPX_OK) return rc;
+  MPX_REQUIRE(out_size >= 1 && out_size <= kMaskMaxM / 2, "mpx_roi_pool: output size %d, must be 1..%d", out_size,
+              kMaskMaxM / 2);
+  if (n == 0) return MPX_OK;
+  MPX_DEVICE(d_pooled);
+  MPX_DEVICE_OR_NULL(d_levels);
+  return roi_pool(h_features, n_images, h, w, h_scales, canonical_scale, canonical_level, sampling, d_boxes, h_counts,
+                  out_size, d_pooled, true, d_levels, static_cast<cudaStream_t>(stream));
+}
+
+static int roi_workspace_ok(const char* fn, const void* d_workspace, size_t workspace_bytes, size_t need) {
+  MPX_REQUIRE(is_device_ptr(d_workspace), "%s: d_workspace is NULL or not device memory", fn);
+  MPX_REQUIRE((reinterpret_cast<uintptr_t>(d_workspace) & 255) == 0, "%s: workspace must be 256-B aligned", fn);
+  MPX_REQUIRE(workspace_bytes >= need, "%s: workspace of %zu bytes < %zu", fn, workspace_bytes, need);
+  return MPX_OK;
+}
+
+int mpx_roi_box_forward(const mpx_roi_heads* heads, const float* const* h_features, int n_images, int h, int w,
+                        const float* h_scales, int canonical_scale, int canonical_level, int sampling,
+                        const float* d_boxes, const int32_t* h_counts, float* d_class_logits, float* d_box_regression,
+                        void* d_workspace, size_t workspace_bytes, void* stream) {
+  MPX_NOT_NULL(heads);
+  long long n = 0;
+  int rc = roi_args_ok(__func__, h_features, n_images, h, w, h_scales, canonical_scale, canonical_level, sampling, d_boxes,
+                       h_counts, &n);
+  if (rc != MPX_OK) return rc;
+  if (n == 0) return MPX_OK;
+  MPX_DEVICE(d_class_logits);
+  MPX_DEVICE(d_box_regression);
+  rc = roi_workspace_ok(__func__, d_workspace, workspace_bytes,
+                        roi_heads_workspace_bytes(heads->heads, static_cast<int>(n), 0, 1));
+  if (rc != MPX_OK) return rc;
+  return roi_box_forward(heads->heads, h_features, n_images, h, w, h_scales, canonical_scale, canonical_level, sampling,
+                         d_boxes, h_counts, d_class_logits, d_box_regression, d_workspace,
+                         static_cast<cudaStream_t>(stream));
+}
+
+int mpx_roi_mask_forward(const mpx_roi_heads* heads, const float* const* h_features, int n_images, int h, int w,
+                         const float* h_scales, int canonical_scale, int canonical_level, int sampling, int mask_pool,
+                         const float* d_boxes, const int32_t* h_counts, float* d_mask_logits, void* d_workspace,
+                         size_t workspace_bytes, void* stream) {
+  MPX_NOT_NULL(heads);
+  long long n = 0;
+  int rc = roi_args_ok(__func__, h_features, n_images, h, w, h_scales, canonical_scale, canonical_level, sampling, d_boxes,
+                       h_counts, &n);
+  if (rc != MPX_OK) return rc;
+  MPX_REQUIRE(mask_pool >= 1 && mask_pool <= kMaskMaxM / 2, "mpx_roi_mask_forward: mask pool %d, must be 1..%d", mask_pool,
+              kMaskMaxM / 2);
+  MPX_REQUIRE(mask_rois_ok(n, mask_pool),
+              "mpx_roi_mask_forward: %lld RoIs of %dx%d: n_rois * 4 * mask_pool^2 must be below 2^31", n, mask_pool,
+              mask_pool);
+  if (n == 0) return MPX_OK;
+  MPX_DEVICE(d_mask_logits);
+  rc = roi_workspace_ok(__func__, d_workspace, workspace_bytes,
+                        roi_heads_workspace_bytes(heads->heads, 0, static_cast<int>(n), mask_pool));
+  if (rc != MPX_OK) return rc;
+  return roi_mask_forward(heads->heads, h_features, n_images, h, w, h_scales, canonical_scale, canonical_level, sampling,
+                          mask_pool, d_boxes, h_counts, d_mask_logits, d_workspace, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -218,6 +218,26 @@ int mask_paste(const float* logits, const long long* labels, const float* boxes,
                int n_images, const int* counts, const int* sizes, float* boxes_out, float* const* masks,
                cudaStream_t stream);
 
+// detector_heads.cu
+struct RoiHeads;
+constexpr int kRoiHeadConvs = 9;  // fc6, fc7, merged predictor, 4 mask-head 3x3, conv5_mask as 1x1, mask_fcn_logits
+constexpr int kRoiBoxPool = 7;    // the box pool's output size (TwoMLPHead on 256 x 7 x 7)
+constexpr int kRoiMaxRois = 1000000;  // RoIs per call (n_rois * 49 pooled pixels stay far below 2^31)
+inline int roi_box_rows(int n_classes) { return (5 * n_classes + 63) / 64 * 64; }
+inline int roi_mask_rows(int n_classes) { return (n_classes + 63) / 64 * 64; }
+int roi_heads_create(const void* const* w, const float* const* b, int n_classes, int hidden, RoiHeads** out);
+void roi_heads_destroy(RoiHeads* h);
+size_t roi_heads_workspace_bytes(const RoiHeads* h, int n_box_rois, int n_mask_rois, int mask_pool);
+int roi_pool(const float* const* features, int n_images, int h, int w, const float* scales, int canonical_scale,
+             int canonical_level, int sampling, const float* boxes, const int* counts, int out_size, void* out, bool f32,
+             int* levels, cudaStream_t stream);
+int roi_box_forward(const RoiHeads* hd, const float* const* features, int n_images, int h, int w, const float* scales,
+                    int canonical_scale, int canonical_level, int sampling, const float* boxes, const int* counts,
+                    float* class_logits, float* box_regression, void* workspace, cudaStream_t stream);
+int roi_mask_forward(const RoiHeads* hd, const float* const* features, int n_images, int h, int w, const float* scales,
+                     int canonical_scale, int canonical_level, int sampling, int s, const float* boxes,
+                     const int* counts, float* mask_logits, void* workspace, cudaStream_t stream);
+
 // raster.cu
 struct MeshDb {
   int n_meshes;

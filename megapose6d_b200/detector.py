@@ -116,14 +116,17 @@ def create_model_detector(cfg, n_classes: int) -> torch.nn.Module:
 
 
 def load_detector(run_id: str, models_root: Optional[Path] = None, device: str = "cuda", engine: bool = False,
-                  device_paste: bool = False) -> Detector:
+                  device_paste: bool = False, engine_roi_heads: bool = False) -> Detector:
     """inference/utils.py:57-70: `<models_root>/<run_id>/{config.yaml, checkpoint.pth.tar}` -> Detector.  `engine=True`
     runs the Mask R-CNN's ResNet-50 FPN backbone and RPN head on the engine's wgmma convolutions
     (`detector_engine.engine_model`; the rest of the model stays torchvision's); with `device_paste=True` as well, the
     mask logits are turned into image-sized masks on the device (`engine_model(..., device_paste=True)`) instead of by
-    torchvision's per-detection loop; the default is torchvision's model throughout, as in the reference."""
-    if device_paste and not engine:
-        raise ValueError("load_detector: device_paste=True needs engine=True")
+    torchvision's per-detection loop; with `engine_roi_heads=True` (implying `device_paste`) the RoI heads' box and mask
+    branches run on the engine too (`engine_model(..., engine_roi_heads=True)`); the default is torchvision's model
+    throughout, as in the reference."""
+    for name, on in (("device_paste", device_paste), ("engine_roi_heads", engine_roi_heads)):
+        if on and not engine:
+            raise ValueError(f"load_detector: {name}=True needs engine=True")
     from . import load_model
 
     run_dir = Path(models_root if models_root is not None else load_model.LOCAL_DATA_DIR / "experiments") / run_id  # EXP_DIR
@@ -137,5 +140,5 @@ def load_detector(run_id: str, models_root: Optional[Path] = None, device: str =
     if engine:
         from .detector_engine import engine_model
 
-        model = engine_model(model, device, device_paste=device_paste)
+        model = engine_model(model, device, device_paste=device_paste, engine_roi_heads=engine_roi_heads)
     return Detector(model)

@@ -221,6 +221,188 @@ def mask_paste(mask_logits: torch.Tensor, labels: torch.Tensor, boxes: torch.Ten
     return list(boxes_out.split(counts)), masks
 
 
+ROI_LEVELS = ["0", "1", "2", "3"]
+ROI_CHANNELS = 256
+BOX_POOL = 7
+MAX_ROWS = 2048  # conv_forward's largest C_out
+
+
+def _rows(n: int) -> int:
+    return (n + 63) // 64 * 64
+
+
+def check_supported_roi_heads(model: nn.Module) -> None:
+    """Raises NotImplementedError for RoI heads `engine_roi_heads=True` does not serve (and for whatever
+    check_supported_device_paste refuses)."""
+    from torchvision.models.detection.faster_rcnn import FastRCNNPredictor, TwoMLPHead
+    from torchvision.models.detection.mask_rcnn import MaskRCNNHeads, MaskRCNNPredictor
+    from torchvision.ops import MultiScaleRoIAlign
+
+    check_supported_device_paste(model)
+    rh = model.roi_heads
+    for name in ("box_roi_pool", "mask_roi_pool"):
+        pool = getattr(rh, name)
+        if type(pool) is not MultiScaleRoIAlign or list(pool.featmap_names) != ROI_LEVELS:
+            _refuse(f"the {name} {type(pool).__name__} (MultiScaleRoIAlign on '0'..'3' only)")
+        if not isinstance(pool.sampling_ratio, int) or pool.sampling_ratio < 1 or pool.sampling_ratio > 16:
+            _refuse(f"the {name} sampling_ratio {pool.sampling_ratio} (a fixed ratio 1..16)")
+        if not isinstance(pool.canonical_scale, int) or not isinstance(pool.canonical_level, int):
+            _refuse(f"the {name} canonical scale / level {pool.canonical_scale} / {pool.canonical_level}")
+    if tuple(rh.box_roi_pool.output_size) != (BOX_POOL, BOX_POOL):
+        _refuse(f"a box pool of {tuple(rh.box_roi_pool.output_size)} (7x7 only)")
+    head = rh.box_head
+    if type(head) is not TwoMLPHead or head.fc6.in_features != ROI_CHANNELS * BOX_POOL * BOX_POOL:
+        _refuse(f"the box head {type(head).__name__} (TwoMLPHead on 256x7x7 only)")
+    hidden = head.fc6.out_features
+    if (hidden % 64 or hidden > MAX_ROWS or head.fc7.in_features != hidden or head.fc7.out_features != hidden
+            or head.fc6.bias is None or head.fc7.bias is None):
+        _refuse(f"a box head of representation size {hidden} (a multiple of 64 up to {MAX_ROWS}, with biases)")
+    pred = rh.box_predictor
+    if type(pred) is not FastRCNNPredictor or pred.cls_score.in_features != hidden:
+        _refuse(f"the box predictor {type(pred).__name__} (FastRCNNPredictor only)")
+    n_classes = pred.cls_score.out_features
+    if pred.bbox_pred.out_features != 4 * n_classes or _rows(5 * n_classes) > MAX_ROWS:
+        _refuse(f"a box predictor of {n_classes} classes (5 x classes rounded up to 64 at most {MAX_ROWS})")
+    mh = rh.mask_head
+    if type(mh) is not MaskRCNNHeads or len(mh) != 4:
+        _refuse(f"the mask head {type(mh).__name__} (MaskRCNNHeads with four layers only)")
+    for i, block in enumerate(mh):
+        conv = block[0] if isinstance(block, nn.Sequential) else None
+        if (not isinstance(conv, nn.Conv2d) or len(block) != 2 or not isinstance(block[1], nn.ReLU)
+                or conv.kernel_size != (3, 3) or conv.stride != (1, 1) or conv.padding != (1, 1)
+                or conv.dilation != (1, 1) or conv.groups != 1 or conv.in_channels != ROI_CHANNELS
+                or conv.out_channels != ROI_CHANNELS or conv.bias is None):
+            _refuse(f"mask head layer {i} (3x3 convolutions of 256 channels with bias and ReLU, no norm)")
+    mp = rh.mask_predictor
+    conv5, logits = getattr(mp, "conv5_mask", None), getattr(mp, "mask_fcn_logits", None)
+    if (type(mp) is not MaskRCNNPredictor or conv5.in_channels != ROI_CHANNELS or conv5.out_channels != ROI_CHANNELS
+            or conv5.padding != (0, 0) or conv5.output_padding != (0, 0) or conv5.groups != 1
+            or conv5.dilation != (1, 1) or conv5.bias is None or not isinstance(logits, nn.Conv2d)
+            or logits.kernel_size != (1, 1) or logits.out_channels != n_classes or logits.bias is None):
+        _refuse(f"the mask predictor {type(mp).__name__} (MaskRCNNPredictor, 256 channels, one logit per class)")
+
+
+def roi_heads_plan(model: nn.Module) -> List[Tuple[torch.Tensor, torch.Tensor]]:
+    """float64 (weight [C_out, R*S*C_in] with k = (r, s, c), bias [C_out]) of the nine convolutions mpx_roi_heads_create
+    takes: fc6 as a 7x7 convolution, fc7, the merged predictor, the four mask-head 3x3, conv5_mask as a 1x1 convolution
+    to the four sub-pixels, mask_fcn_logits.  The predictors are zero-padded to a multiple of 64 rows."""
+    rh = model.roi_heads
+    d = lambda t: t.detach().double().cpu()  # noqa: E731
+
+    def pad(w, b):
+        rows = _rows(w.shape[0])
+        return (torch.cat([w, w.new_zeros(rows - w.shape[0], w.shape[1])]),
+                torch.cat([b, b.new_zeros(rows - b.shape[0])]))
+
+    fc6, fc7 = rh.box_head.fc6, rh.box_head.fc7
+    hidden = fc6.out_features
+    plan = [(_pack(d(fc6.weight).view(hidden, ROI_CHANNELS, BOX_POOL, BOX_POOL)), d(fc6.bias)),
+            (d(fc7.weight), d(fc7.bias))]
+    pred = rh.box_predictor
+    plan.append(pad(torch.cat([d(pred.cls_score.weight), d(pred.bbox_pred.weight)]),
+                    torch.cat([d(pred.cls_score.bias), d(pred.bbox_pred.bias)])))
+    plan += [(_pack(d(block[0].weight)), d(block[0].bias)) for block in rh.mask_head]
+    conv5, logits = rh.mask_predictor.conv5_mask, rh.mask_predictor.mask_fcn_logits
+    # ConvTranspose2d weight [in, out, dy, dx] -> row (dy * 2 + dx) * out + o, column = input channel
+    plan.append((d(conv5.weight).permute(2, 3, 1, 0).reshape(4 * ROI_CHANNELS, ROI_CHANNELS), d(conv5.bias).repeat(4)))
+    plan.append(pad(d(logits.weight).flatten(1), d(logits.bias)))
+    return plan
+
+
+def pool_args(pool: nn.Module, features: List[torch.Tensor], image_sizes: List[Tuple[int, int]]):
+    """(scales, canonical_scale, canonical_level, sampling_ratio) as MultiScaleRoIAlign computes them for these features
+    and images (torchvision.ops.poolers._setup_scales), without caching them in the module."""
+    from torchvision.ops.poolers import _setup_scales
+
+    scales, _ = _setup_scales(features, image_sizes, pool.canonical_scale, pool.canonical_level)
+    return (ctypes.c_float * 4)(*scales), pool.canonical_scale, pool.canonical_level, pool.sampling_ratio
+
+
+class RoiHeadsEngine:
+    """Owns the repacked device weights of the RoI heads and the mpx_roi_heads handle (include/mpx.h)."""
+
+    def __init__(self, model: nn.Module, device="cuda"):
+        check_supported_roi_heads(model)
+        rh = model.roi_heads
+        self.device = torch.device(device)
+        self.n_classes = rh.box_predictor.cls_score.out_features
+        self.hidden = rh.box_head.fc6.out_features
+        self.mask_pool = int(rh.mask_roi_pool.output_size[0])
+        self._box_pool, self._mask_pool = rh.box_roi_pool, rh.mask_roi_pool
+        act = _abi.act_dtype()
+        plan = roi_heads_plan(model)
+        self._weights = [to_act16(w, act).to(self.device).contiguous() for w, _ in plan]
+        self._biases = [b.to(torch.float32).to(self.device).contiguous() for _, b in plan]
+        n = len(self._weights)
+        wp = (ctypes.c_void_p * n)(*[t.data_ptr() for t in self._weights])
+        bp = (ctypes.c_void_p * n)(*[t.data_ptr() for t in self._biases])
+        handle = ctypes.c_void_p()
+        _abi.check(_abi.lib().mpx_roi_heads_create(wp, bp, n, self.n_classes, self.hidden, ctypes.byref(handle)))
+        self._handle = handle
+        self._workspace: Optional[torch.Tensor] = None
+
+    def __del__(self):
+        try:
+            if getattr(self, "_handle", None) is not None:
+                _abi.lib().mpx_roi_heads_destroy(self._handle)
+        except Exception:  # noqa: BLE001
+            pass
+
+    def _ws(self, n_box: int, n_mask: int) -> torch.Tensor:
+        need = _abi.lib().mpx_roi_heads_workspace_bytes(self._handle, n_box, n_mask, self.mask_pool)
+        if self._workspace is None or self._workspace.numel() < need:
+            self._workspace = None
+            self._workspace = torch.empty(max(need, 256), dtype=torch.uint8, device=self.device)
+        return self._workspace
+
+    def _features(self, features, n_images: int, batch_hw: Tuple[int, int]) -> Tuple[List[torch.Tensor], "ctypes.Array"]:
+        """The levels '0'..'3', checked against the shapes the kernels derive from the batch size and count."""
+        feats = [features[k] for k in ROI_LEVELS]
+        for l, f in enumerate(feats):
+            want = (n_images, ROI_CHANNELS, batch_hw[0] >> (l + 2), batch_hw[1] >> (l + 2))
+            if f.dtype != torch.float32 or not f.is_contiguous() or tuple(f.shape) != want or not f.is_cuda:
+                raise ValueError(f"RoiHeadsEngine: level {l} must be a contiguous fp32 CUDA tensor {list(want)}, "
+                                 f"got {f.dtype} {tuple(f.shape)} on {f.device}")
+        return feats, (ctypes.c_void_p * 4)(*[f.data_ptr() for f in feats])
+
+    def _boxes(self, boxes: torch.Tensor, n: int) -> torch.Tensor:
+        if tuple(boxes.shape) != (n, 4) or not boxes.is_cuda:
+            raise ValueError(f"RoiHeadsEngine: boxes must be a CUDA tensor [{n}, 4], got {tuple(boxes.shape)} on "
+                             f"{boxes.device}")
+        return boxes.to(torch.float32).contiguous()
+
+    def box(self, features, boxes: torch.Tensor, counts: List[int], batch_hw: Tuple[int, int],
+            image_sizes: List[Tuple[int, int]]) -> Tuple[torch.Tensor, torch.Tensor]:
+        """box_roi_pool + box_head + box_predictor: fp32 class_logits [P, C] and box_regression [P, 4C] of the RoIs
+        `boxes` [P, 4] (counts: RoIs per image)."""
+        feats, fp = self._features(features, len(counts), batch_hw)
+        n = int(sum(counts))
+        boxes = self._boxes(boxes, n)
+        logits = torch.empty(n, self.n_classes, device=self.device)
+        deltas = torch.empty(n, 4 * self.n_classes, device=self.device)
+        ws = self._ws(n, 0)
+        _abi.check(_abi.lib().mpx_roi_box_forward(
+            self._handle, fp, len(counts), batch_hw[0], batch_hw[1], *pool_args(self._box_pool, feats, image_sizes),
+            boxes.data_ptr(), (ctypes.c_int32 * len(counts))(*counts), logits.data_ptr(), deltas.data_ptr(),
+            ws.data_ptr(), ws.numel(), _abi.stream_ptr()))
+        return logits, deltas
+
+    def mask(self, features, boxes: torch.Tensor, counts: List[int], batch_hw: Tuple[int, int],
+             image_sizes: List[Tuple[int, int]]) -> torch.Tensor:
+        """mask_roi_pool + mask_head + mask_predictor: fp32 mask logits [N, C, 2s, 2s] of the boxes [N, 4]."""
+        feats, fp = self._features(features, len(counts), batch_hw)
+        n = int(sum(counts))
+        m = 2 * self.mask_pool
+        boxes = self._boxes(boxes, n)
+        out = torch.empty(n, self.n_classes, m, m, device=self.device)
+        ws = self._ws(0, n)
+        _abi.check(_abi.lib().mpx_roi_mask_forward(
+            self._handle, fp, len(counts), batch_hw[0], batch_hw[1], *pool_args(self._mask_pool, feats, image_sizes),
+            self.mask_pool, boxes.data_ptr(), (ctypes.c_int32 * len(counts))(*counts), out.data_ptr(), ws.data_ptr(),
+            ws.numel(), _abi.stream_ptr()))
+        return out
+
+
 class FpnEngine:
     """Owns the repacked device weights and the mpx_fpn handle.  `run(images)` returns the FPN features, objectness and
     deltas of a padded fp32 batch [n, 3, h, w] as lists of five fp32 NCHW tensors.  The tensors are the engine's own
@@ -282,12 +464,17 @@ class EngineMaskRCNN(nn.Module):
     """Called like torchvision's GeneralizedRCNN in eval mode: `module(images)` -> list of dicts(boxes, labels, scores,
     masks).  Holds the model's transform, RPN and RoI heads by reference (not as submodules: it does not own them)."""
 
-    def __init__(self, model: nn.Module, device="cuda", device_paste: bool = False):
+    def __init__(self, model: nn.Module, device="cuda", device_paste: bool = False, engine_roi_heads: bool = False):
         super().__init__()
-        if device_paste:
+        device_paste = device_paste or engine_roi_heads
+        if engine_roi_heads:
+            check_supported_roi_heads(model)
+        elif device_paste:
             check_supported_device_paste(model)
         self.device_paste = device_paste
+        self.engine_roi_heads = engine_roi_heads
         self.engine = FpnEngine(model, device)
+        self.roi_engine = RoiHeadsEngine(model, device) if engine_roi_heads else None
         self._stages = (model.transform, model.rpn, model.roi_heads)
         for attr in ("config", "cfg"):
             if hasattr(model, attr):
@@ -329,6 +516,9 @@ class EngineMaskRCNN(nn.Module):
         if not self.device_paste:
             detections, _ = roi_heads(features, proposals, image_list.image_sizes)
             return transform.postprocess(detections, image_list.image_sizes, original_image_sizes)
+        if self.engine_roi_heads:
+            return self.detect_engine(features, proposals, tuple(image_list.tensors.shape[-2:]), image_list.image_sizes,
+                                      original_image_sizes)
         return self.detect(features, proposals, image_list.image_sizes, original_image_sizes)
 
     def detect(self, features, proposals, image_sizes, original_image_sizes) -> List[Dict[str, torch.Tensor]]:
@@ -345,12 +535,33 @@ class EngineMaskRCNN(nn.Module):
         return [dict(boxes=b, labels=l, scores=s, masks=m) for b, l, s, m in zip(boxes, labels, scores, masks)]
 
 
-def engine_model(model: nn.Module, device="cuda", device_paste: bool = False) -> EngineMaskRCNN:
+    def detect_engine(self, features, proposals, batch_hw, image_sizes, original_image_sizes
+                      ) -> List[Dict[str, torch.Tensor]]:
+        """`detect` with the box and mask branches on the engine (`RoiHeadsEngine`) and the model's
+        postprocess_detections between them."""
+        rh = self._stages[2]
+        counts = [int(p.shape[0]) for p in proposals]
+        class_logits, box_regression = self.roi_engine.box(features, torch.cat(proposals), counts, batch_hw, image_sizes)
+        boxes, scores, labels = rh.postprocess_detections(class_logits, box_regression, proposals, image_sizes)
+        counts = [int(b.shape[0]) for b in boxes]
+        boxes_cat = torch.cat(boxes)
+        mask_logits = self.roi_engine.mask(features, boxes_cat, counts, batch_hw, image_sizes)
+        boxes, masks = mask_paste(mask_logits, torch.cat(labels), boxes_cat, counts, image_sizes, original_image_sizes)
+        return [dict(boxes=b, labels=l, scores=s, masks=m) for b, l, s, m in zip(boxes, labels, scores, masks)]
+
+
+def engine_model(model: nn.Module, device="cuda", device_paste: bool = False,
+                 engine_roi_heads: bool = False) -> EngineMaskRCNN:
     """`model` (a torchvision MaskRCNN on `device`, in eval mode) with its backbone and RPN head on the engine.  Raises
     NotImplementedError, before any device work, for a structure the plan does not serve: a backbone other than the
     ResNet-50 body with FPN (returned layers 1-4, 256 channels, LastLevelMaxPool), a norm other than FrozenBatchNorm2d,
     dilation, an RPN head with conv_depth != 1 or more than 12 anchors per location, size_divisible != 32.
     `device_paste=True` also pastes the masks on the device (`mask_paste`) and refuses, likewise, RoI heads without a mask
     branch or with a keypoint branch, non-square mask pools, a mask predictor other than a 2x2/2 ConvTranspose2d and
-    masks larger than 64x64, and a transform other than GeneralizedRCNNTransform."""
-    return EngineMaskRCNN(model, device, device_paste)
+    masks larger than 64x64, and a transform other than GeneralizedRCNNTransform.  `engine_roi_heads=True` implies
+    `device_paste=True` and runs the box and mask branches on the engine (`RoiHeadsEngine`); it refuses as well pools
+    other than MultiScaleRoIAlign on '0'..'3' with a fixed sampling ratio, a box pool other than 7x7, a box head other
+    than TwoMLPHead on 256x7x7, a box predictor other than FastRCNNPredictor or with 5 x classes above 2048 rows, a mask
+    head other than MaskRCNNHeads (four 3x3 convolutions of 256 channels, no norm, ReLU) and a mask predictor other than
+    MaskRCNNPredictor."""
+    return EngineMaskRCNN(model, device, device_paste, engine_roi_heads)

@@ -508,7 +508,11 @@ def main(argv: Optional[List[str]] = None) -> None:
                         help="run the detector's ResNet-50 FPN backbone and RPN head on the engine's convolutions")
     parser.add_argument("--detector-device-paste", action="store_true",
                         help="as --detector-engine, and turn the detector's mask logits into image-sized masks on the device")
+    parser.add_argument("--detector-engine-roi-heads", action="store_true",
+                        help="as --detector-device-paste, and run the detector's RoI box and mask branches on the engine")
     args = parser.parse_args(argv)
+    if args.detector_engine_roi_heads:
+        args.detector_device_paste = True
     if args.detector_device_paste:
         args.detector_engine = True
     if args.detector_engine and args.detector is None:
@@ -549,7 +553,8 @@ def main(argv: Optional[List[str]] = None) -> None:
         from .detector import load_detector
 
         pose_estimator.detector_model = load_detector(args.detector, models_root=args.models_root,
-                                                      engine=args.detector_engine, device_paste=args.detector_device_paste)
+                                                      engine=args.detector_engine, device_paste=args.detector_device_paste,
+                                                      engine_roi_heads=args.detector_engine_roi_heads)
     out = run_predictions(scene_ds, pose_estimator, cfg, save_dir=args.save_dir)
     if out["save_dir"] is not None:
         n = len(out["results"]["predictions"]["final"])

@@ -4,6 +4,8 @@ Workload: the seeded detector of `workloads.detector.make_detector` (no trained 
 batch 1 and 8, with `input_resize` (480, 640) and the reference default (240, 320).  Arms:
   engine     backbone + RPN head as one mpx_fpn_forward (detector_engine.engine_model), the rest torchvision fp32
   engine_paste  as engine, and the masks pasted on the device (engine_model(..., device_paste=True): one mpx_mask_paste)
+  engine_heads  as engine_paste, and the RoI heads' box and mask branches on the engine (engine_model(...,
+             engine_roi_heads=True): mpx_roi_box_forward, torchvision's postprocess_detections, mpx_roi_mask_forward)
   fp32       torchvision, TF32 off
   tf32       torchvision with torch's defaults (cuDNN convolutions in TF32)
   fp16_cl    torchvision under fp16 autocast, channels_last
@@ -11,7 +13,8 @@ Stages: `heads` = backbone + RPN head (one mpx_fpn_forward for the engine), `res
 postprocessing from those outputs, `detector` = the whole `Detector.get_detections`.  `rest` is split, on the engine's
 head outputs, into torchvision's `proposals` (anchors, decoding, filter_proposals), `box` (box RoI pool, box head, box
 predictor, postprocess_detections), `mask` (mask RoI pool, mask head, mask predictor) and `paste` (maskrcnn_inference and
-GeneralizedRCNNTransform.postprocess), next to `paste_engine` (mpx_mask_paste).  After a warm-up, every window times
+GeneralizedRCNNTransform.postprocess), next to the engine's `box_engine` (mpx_roi_box_forward and the same
+postprocess_detections), `mask_engine` (mpx_roi_mask_forward) and `paste_engine` (mpx_mask_paste).  After a warm-up, every window times
 each arm in turn (CUDA events, `--calls` calls) and the medians over `--windows` windows are reported, with the engine's
 convolution TFLOP/s (mpx_profile_enable: events around every convolution, FLOPs from the shapes), the largest per-level
 relative error of each arm's head outputs against fp32, the device name and its power limit, as one JSON line.
@@ -61,7 +64,7 @@ def arm_context(arm: str):
     return contextlib.nullcontext()
 
 
-def split_stages(model, engine, image_list, batch: int):
+def split_stages(model, engine, roi, image_list, batch: int):
     """torchvision's stages after the RPN head, one by one, each fed the previous stage's outputs computed once from the
     engine's head outputs; and the device paste on the same inputs."""
     rh, sizes, orig = model.roi_heads, image_list.image_sizes, [(480, 640)] * batch
@@ -95,7 +98,20 @@ def split_stages(model, engine, image_list, batch: int):
     def paste_engine():
         return E.mask_paste(logits, torch.cat(labels), torch.cat(boxes), counts, sizes, orig)
 
-    return dict(proposals=proposals, box=box, mask=mask, paste=paste, paste_engine=paste_engine), counts
+    hw = tuple(image_list.tensors.shape[-2:])
+    n_props = [int(p.shape[0]) for p in props]
+    props_cat, boxes_cat = torch.cat(props), torch.cat(boxes)
+
+    def box_engine():
+        with torch.no_grad():
+            c, r = roi.box(feats, props_cat, n_props, hw, sizes)
+            return rh.postprocess_detections(c, r, props, sizes)
+
+    def mask_engine():
+        return roi.mask(feats, boxes_cat, counts, hw, sizes)
+
+    return dict(proposals=proposals, box=box, mask=mask, paste=paste, box_engine=box_engine, mask_engine=mask_engine,
+                paste_engine=paste_engine), counts
 
 
 def main() -> None:
@@ -112,16 +128,17 @@ def main() -> None:
         cl = copy.deepcopy(model).to(memory_format=torch.channels_last)
         engine = E.engine_model(model)
         engine_paste = E.engine_model(model, device_paste=True)
+        engine_heads = E.engine_model(model, engine_roi_heads=True)
         tv = {"fp32": model, "tf32": model, "fp16_cl": cl}
         for batch in (1, 8):
             g = torch.Generator().manual_seed(batch)
             images = torch.rand(batch, 3, 480, 640, generator=g).cuda()
             obs = ObservationTensor(images, torch.eye(3).repeat(batch, 1, 1).cuda())
             image_list, _ = model.transform(list(images))
-            arms = ["engine", "engine_paste", "fp32", "tf32", "fp16_cl"]
+            arms = ["engine", "engine_paste", "engine_heads", "fp32", "tf32", "fp16_cl"]
             heads_out, fns = {}, {}
             for arm in arms:
-                m = {"engine": engine, "engine_paste": engine_paste}.get(arm) or tv[arm]
+                m = {"engine": engine, "engine_paste": engine_paste, "engine_heads": engine_heads}.get(arm) or tv[arm]
                 det = Detector(m)
 
                 def heads(arm=arm):
@@ -145,6 +162,9 @@ def main() -> None:
                         props = engine.proposals(image_list, feats, o, d)
                         if arm == "engine_paste":
                             return engine_paste.detect(feats, props, image_list.image_sizes, [(480, 640)] * batch)
+                        if arm == "engine_heads":
+                            return engine_heads.detect_engine(feats, props, tuple(image_list.tensors.shape[-2:]),
+                                                              image_list.image_sizes, [(480, 640)] * batch)
                         r = tv[arm] if not arm.startswith("engine") else model
                         dets, _ = r.roi_heads(feats, props, image_list.image_sizes)
                         return r.transform.postprocess(dets, image_list.image_sizes, [(480, 640)] * batch)
@@ -154,7 +174,7 @@ def main() -> None:
                         return det.get_detections(obs)
 
                 fns[arm] = dict(heads=heads, rest=rest, detector=whole)
-            fns["split"], counts = split_stages(model, engine, image_list, batch)
+            fns["split"], counts = split_stages(model, engine, engine_heads.roi_engine, image_list, batch)
             for arm in arms:  # warm-up: algorithm selection, graph capture
                 for fn in fns[arm].values():
                     for _ in range(3):
@@ -184,6 +204,7 @@ def main() -> None:
                         heads_speedup_vs_fp16_cl=med["fp16_cl"]["heads"] / med["engine"]["heads"],
                         detector_speedup_vs_fp32=med["fp32"]["detector"] / med["engine"]["detector"],
                         detector_speedup_paste_vs_engine=med["engine"]["detector"] / med["engine_paste"]["detector"],
+                        detector_speedup_heads_vs_paste=med["engine_paste"]["detector"] / med["engine_heads"]["detector"],
                         detections=counts)
             out["cases"].append(case)
             print(json.dumps(case), file=sys.stderr, flush=True)

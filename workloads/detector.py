@@ -119,3 +119,32 @@ def integer_weights(model: torch.nn.Module, seed: int = 0, nnz: int = 2) -> torc
             m.running_var.fill_(1.0)
             m.eps = 0.0
     return model
+
+
+@torch.no_grad()
+def integer_roi_heads_weights(model: torch.nn.Module, seed: int = 0, nnz: int = 2) -> torch.nn.Module:
+    """In place: every layer of the RoI heads (fc6, fc7, cls_score, bbox_pred, the mask head's convolutions,
+    conv5_mask and mask_fcn_logits) gets `nnz` weights of +-1 per output row (the rest zero) and an integer bias in
+    -2..2.  Each output is then a sum of nnz act16 inputs and an integer, which fp32 accumulates exactly in any order
+    for inputs of small dynamic range, so only the one rounding per layer remains between the engine and the float64
+    oracle (oracle/detector_heads_ref.py)."""
+    rh = model.roi_heads
+    g = torch.Generator().manual_seed(seed)
+    layers = [rh.box_head.fc6, rh.box_head.fc7, rh.box_predictor.cls_score, rh.box_predictor.bbox_pred,
+              *[block[0] for block in rh.mask_head], rh.mask_predictor.mask_fcn_logits]
+    for m in layers:
+        co = m.weight.shape[0]
+        k = m.weight[0].numel()
+        w = torch.zeros(co, k)
+        idx = torch.stack([torch.randperm(k, generator=g)[:nnz] for _ in range(co)])
+        w.scatter_(1, idx, (torch.randint(0, 2, (co, nnz), generator=g) * 2 - 1).float())
+        m.weight.copy_(w.view_as(m.weight))
+        m.bias.copy_(torch.randint(-2, 3, (co,), generator=g).float())
+    conv5 = rh.mask_predictor.conv5_mask  # weight [in, out, 2, 2]: nnz input channels per (output channel, tap)
+    ci, co = conv5.weight.shape[:2]
+    w = torch.zeros(co * 4, ci)
+    idx = torch.stack([torch.randperm(ci, generator=g)[:nnz] for _ in range(co * 4)])
+    w.scatter_(1, idx, (torch.randint(0, 2, (co * 4, nnz), generator=g) * 2 - 1).float())
+    conv5.weight.copy_(w.view(co, 2, 2, ci).permute(3, 0, 1, 2))
+    conv5.bias.copy_(torch.randint(-2, 3, (co,), generator=g).float())
+    return model
